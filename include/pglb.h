@@ -131,6 +131,17 @@ int pglb_spmm_csr_f32(const int64_t *indptr, const int64_t *cols, const int64_t 
                       int reduce_op, const float *scale_src, const float *scale_dst,
                       const uint32_t *cols_packed, int64_t max_degree_hint, int flags, void *ws,
                       size_t ws_bytes, void *stream);
+/* pglb_spmm_csr_f32 plus scale_slot[E] (nullable, wins over scale_src): the source scale already laid out per CSR
+ * slot (scale_slot[j] = scale_src[cols[j]]), streamed by the wide-row kernel instead of gathered, which would cost a
+ * 32-byte sector per edge.  The kernels that do not stream it gather scale_src, so scale_slot needs scale_src
+ * (PGLB_EINVAL otherwise).  pglb_spmm_csr_f32 is this call with scale_slot = NULL.  Same results either way. */
+int pglb_spmm_csr_slot_scale_f32(const int64_t *indptr, const int64_t *cols, const int64_t *eid,
+                                 const float *x, int64_t ldx, const float *y, int64_t ldy, int y_bcast,
+                                 float *out, int64_t ldo, int64_t n_dst, int64_t n_src,
+                                 int64_t num_edges, int64_t D, int64_t head_dim, int msg_op,
+                                 int reduce_op, const float *scale_src, const float *scale_slot,
+                                 const float *scale_dst, const uint32_t *cols_packed, int64_t max_degree_hint,
+                                 int flags, void *ws, size_t ws_bytes, void *stream);
 /* flags of pglb_spmm_csr_f32 */
 #define PGLB_SPMM_ACCUMULATE 1 /* SUM only: out[d] = (out[d] + sum of messages) * scale_dst[d];
                                   lets a caller aggregate one edge subset while the feature rows of

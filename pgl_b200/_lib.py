@@ -47,6 +47,9 @@ _SIGS = {
     "pglb_spmm_csr_ws": (c_int, [_i64, _i64, _i64, POINTER(c_size_t)]),
     "pglb_spmm_csr_f32": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, c_int, _p, _i64, _i64, _i64, _i64,
                                   _i64, _i64, c_int, c_int, _p, _p, _p, _i64, c_int, _p, c_size_t, _p]),
+    "pglb_spmm_csr_slot_scale_f32": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, c_int, _p, _i64, _i64, _i64, _i64,
+                                             _i64, _i64, c_int, c_int, _p, _p, _p, _p, _i64, c_int, _p, c_size_t,
+                                             _p]),
     "pglb_narrow_plan_ws": (c_int, [_i64, POINTER(c_size_t)]),
     "pglb_narrow_plan": (c_int, [_p, _p, _p, _i64, _i64, _i64, _p, _p, _p, _p, c_size_t, _p]),
     "pglb_spmm_narrow_ws": (c_int, [_i64, _i64, POINTER(c_size_t)]),

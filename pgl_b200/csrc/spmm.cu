@@ -416,7 +416,7 @@ static inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t
 size_t stream_ws_bytes(int64_t E, int64_t D);
 int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, int64_t ldx,
                     float *out, int64_t ldo, int64_t n_dst, int64_t n_src, int64_t E, int64_t D,
-                    int reduce_op, const float *scale_src, const float *scale_dst,
+                    int reduce_op, const float *scale_src, const float *scale_slot, const float *scale_dst,
                     const uint32_t *cols32, int l2_hints, int accumulate, const int64_t *eid,
                     const float *y, int64_t ldy, int y_bcast, int head_dim, int msg_op, void *ws,
                     size_t ws_bytes, cudaStream_t stream);
@@ -459,6 +459,19 @@ extern "C" int pglb_spmm_csr_f32(const int64_t *indptr, const int64_t *cols, con
                                  const float *scale_dst, const uint32_t *cols_packed,
                                  int64_t max_degree_hint, int flags, void *ws, size_t ws_bytes,
                                  void *stream_) {
+    return pglb_spmm_csr_slot_scale_f32(indptr, cols, eid, x, ldx, y, ldy, y_bcast, out, ldo, n_dst, n_src, num_edges,
+                                        D, head_dim, msg_op, reduce_op, scale_src, nullptr, scale_dst, cols_packed,
+                                        max_degree_hint, flags, ws, ws_bytes, stream_);
+}
+
+extern "C" int pglb_spmm_csr_slot_scale_f32(const int64_t *indptr, const int64_t *cols, const int64_t *eid,
+                                            const float *x, int64_t ldx, const float *y, int64_t ldy,
+                                            int y_bcast, float *out, int64_t ldo, int64_t n_dst,
+                                            int64_t n_src, int64_t num_edges, int64_t D, int64_t head_dim,
+                                            int msg_op, int reduce_op, const float *scale_src,
+                                            const float *scale_slot, const float *scale_dst,
+                                            const uint32_t *cols_packed, int64_t max_degree_hint, int flags,
+                                            void *ws, size_t ws_bytes, void *stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     PGLB_CHECK_ARG(n_dst >= 0 && n_src >= 0 && num_edges >= 0 && D >= 0, PGLB_EINVAL,
                    "pglb_spmm_csr_f32: negative size");
@@ -466,6 +479,7 @@ extern "C" int pglb_spmm_csr_f32(const int64_t *indptr, const int64_t *cols, con
                    "pglb_spmm_csr_f32: unknown reduce_op %d", reduce_op);
     PGLB_CHECK_ARG(msg_op >= PGLB_MSG_COPY && msg_op <= PGLB_MSG_DIV, PGLB_EINVAL,
                    "pglb_spmm_csr_f32: unknown msg_op %d", msg_op);
+    PGLB_CHECK_ARG(!scale_slot || scale_src, PGLB_EINVAL, "pglb_spmm_csr_slot_scale_f32: scale_slot needs scale_src");
     if (n_dst == 0 || D == 0) return PGLB_OK;
     PGLB_CHECK_ARG(indptr && out, PGLB_EINVAL, "pglb_spmm_csr_f32: indptr/out is NULL");
     PGLB_CHECK_ARG(num_edges == 0 || x, PGLB_EINVAL, "pglb_spmm_csr_f32: x is NULL");
@@ -497,7 +511,7 @@ extern "C" int pglb_spmm_csr_f32(const int64_t *indptr, const int64_t *cols, con
         PGLB_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
                        "pglb_spmm_csr_f32: workspace must be 256-byte aligned");
         return spmm_stream_run(indptr, cols, x, ldx, out, ldo, n_dst, n_src, num_edges, D,
-                               reduce_op, scale_src, scale_dst, mode == 0 ? cols_packed : nullptr,
+                               reduce_op, scale_src, scale_slot, scale_dst, mode == 0 ? cols_packed : nullptr,
                                (flags & PGLB_SPMM_L2_HINTS) ? 1 : 0, accumulate, eid,
                                mode == 1 ? y : nullptr, ldy, y_bcast, (int)head_dim, msg_op, ws,
                                ws_bytes, stream);

@@ -46,6 +46,7 @@ struct StreamP {
     int reduce_op;
     const float *scale_src;
     const float *scale_dst;
+    const float *scale_slot;  // nullable [E]: scale_src[cols[j]] per slot, streamed by spmm_v5 instead of gathered
     int64_t T;  // nominal slots per task (multiple of 32)
     int64_t ntasks;
     const int64_t *first_row;  // [ntasks]
@@ -101,6 +102,9 @@ __device__ __forceinline__ float lds32(unsigned addr) {
     float v;
     asm volatile("ld.shared.f32 %0, [%1];\n" : "=f"(v) : "r"(addr));
     return v;
+}
+__device__ __forceinline__ void sts32(unsigned addr, float v) {
+    asm volatile("st.shared.f32 [%0], %1;\n" ::"r"(addr), "f"(v) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
 template <int N>
@@ -1234,7 +1238,7 @@ static int launch_stream(const StreamP &p, int tiles, cudaStream_t stream) {
 // Called by pglb_spmm_csr_f32 for the eligible shapes.  `ws` holds >= stream_ws_bytes().
 int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, int64_t ldx,
                     float *out, int64_t ldo, int64_t n_dst, int64_t n_src, int64_t E, int64_t D,
-                    int reduce_op, const float *scale_src, const float *scale_dst,
+                    int reduce_op, const float *scale_src, const float *scale_slot, const float *scale_dst,
                     const uint32_t *cols32, int l2_hints, int accumulate, const int64_t *eid,
                     const float *y, int64_t ldy, int y_bcast, int head_dim, int msg_op, void *ws,
                     size_t ws_bytes, cudaStream_t stream) {
@@ -1256,6 +1260,7 @@ int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, 
     p.reduce_op = reduce_op;
     p.scale_src = scale_src;
     p.scale_dst = scale_dst;
+    p.scale_slot = scale_slot;  // spmm_v5 only; the other kernels below gather scale_src
     p.T = T;
     p.ntasks = w.ntasks;
     p.first_row = w.first_row;

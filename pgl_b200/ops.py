@@ -3,6 +3,7 @@ torch, passes raw device pointers + the current CUDA stream to libpglb.  CUDA te
 every function raises on CPU tensors; there is no eager / CPU fallback on this path.
 """
 import ctypes
+import functools
 import os
 
 import torch
@@ -287,11 +288,16 @@ def _spmm_raw(indptr, cols, x2, n_dst, reduce_op, eid=None, y2=None, y_bcast=BCA
     check(lib.pglb_spmm_csr_ws(n_dst, E, D, ctypes.byref(need)))
     ws = workspace(dev, need.value)
     wsn = ws.numel()
+    sslot = None
+    if (scale_src is not None and reduce_op in ("sum", "mean") and msg_op == "copy"
+            and getattr(packed, "slot_scale", None) is not None):
+        # scale_src[cols[j]] per slot (None before the scale's second call) for spmm_v5, the kernel of these calls
+        sslot = packed.slot_scale(scale_src)
     with torch.cuda.device(dev):
-        check(lib.pglb_spmm_csr_f32(
+        check(lib.pglb_spmm_csr_slot_scale_f32(
             _ptr(indptr), _ptr(cols), _ptr(eid), _ptr(x2), x2.stride(0), _ptr(y2),
             (y2.stride(0) if y2 is not None else 0), y_bcast, _ptr(out), out.stride(0), n_dst,
-            int(x2.shape[0]), E, D, head_dim, MSG[msg_op], REDUCE[reduce_op], _ptr(scale_src),
+            int(x2.shape[0]), E, D, head_dim, MSG[msg_op], REDUCE[reduce_op], _ptr(scale_src), _ptr(sslot),
             _ptr(scale_dst), _ptr(packed[0]) if packed is not None else None, int(max_degree),
             (1 if accumulate else 0) | (2 if (packed is not None and packed[1]) else 0), _ptr(ws),
             wsn, _stream()))
@@ -465,15 +471,45 @@ def gather_rows_ptr(src_ptr, ld, index, out):
     return out
 
 
-HOT_L2_BYTES = int(float(os.environ.get("PGLB_HOT_MB", "64")) * (1 << 20))
+# Share of the device's L2 given to the rows marked evict_last (the "hot set") of the wide-row kernel: 32 MB of an
+# H100's 50 MB.  The rest of the cache holds what streams past it: packed ids, per-slot norms, output write-back and
+# the cold rows in flight.  scripts/l2_sweep.py on cfg5 (DESIGN.md section 6) found the step time flat within 0.1 %
+# from 24 to 64 MB with streamed norms and 32 MB the lowest median; no budget at all costs about 1 %.
+HOT_L2_FRACTION = 0.64
+
+
+@functools.lru_cache(maxsize=None)
+def _l2_bytes(device_index):
+    return int(torch.cuda.get_device_properties(device_index).L2_cache_size)
+
+
+def hot_l2_bytes(device):
+    """L2 budget of the wide-row hot set on `device`: PGLB_HOT_MB when set (0 = no hints), else HOT_L2_FRACTION of
+    the device's L2."""
+    env = os.environ.get("PGLB_HOT_MB")
+    if env is not None:
+        return int(float(env) * (1 << 20))
+    dev = torch.device(device)
+    return int(HOT_L2_FRACTION * _l2_bytes(dev.index if dev.index is not None else torch.cuda.current_device()))
+
+
+class PackedCols(tuple):
+    """(packed uint32 column ids, has_hints) of pack_cols for the wide-row kernel, plus `slot_scale(scale_src)`: the
+    EdgeIndex's per-slot source scale (None until a scale tensor's second call), which the kernel streams instead
+    of gathering scale_src per edge."""
+
+    def __new__(cls, packed, slot_scale=None):
+        self = tuple.__new__(cls, packed)
+        self.slot_scale = slot_scale
+        return self
 
 
 def pack_cols(cols, n_src, row_bytes, budget_bytes=None):
     """(packed uint32 column ids, has_hints) for the wide-row aggregation kernel, or None when
-    ids do not fit 31 bits.  With a budget (PGLB_HOT_MB, default 32 MB; 0 = no hints) bit 31 marks the
+    ids do not fit 31 bits.  With a budget (default hot_l2_bytes(cols.device); 0 = no hints) bit 31 marks the
     most frequently gathered sources, as many as fit in the budget, for an evict_last L2 policy.
     One-off per graph; cached by EdgeIndex."""
-    budget = HOT_L2_BYTES if budget_bytes is None else int(budget_bytes)
+    budget = hot_l2_bytes(cols.device) if budget_bytes is None else int(budget_bytes)
     n_src = int(n_src)
     E = int(cols.shape[0])
     if n_src >= (1 << 31) - 1 or E == 0 or n_src == 0:
@@ -614,7 +650,8 @@ def _packed_of(csr, x2):
                           fallback=(lambda: fn(n_src, D * 4)) if NARROW_ROWS else None)
     if D <= 64 and not NARROW_ROWS:
         return None
-    return fn(n_src, D * 4)
+    pk = fn(n_src, D * 4)
+    return PackedCols(pk, csr.get("slot_scale")) if pk is not None else None
 
 
 @f64_through

@@ -119,9 +119,10 @@ class EdgeIndex(object):
     def packed_cols(self, n_src, row_bytes):
         """Cached packed column ids (see ops.pack_cols) for gathers of `row_bytes` rows."""
         cache = self.__dict__.setdefault("_packed_cache", {})
-        key = (int(n_src), int(row_bytes) if ops.HOT_L2_BYTES > 0 else 0)
+        budget = ops.hot_l2_bytes(self._sorted_v.device)
+        key = (int(n_src), int(row_bytes), budget)
         if key not in cache:
-            cache[key] = ops.pack_cols(self._sorted_v, n_src, row_bytes)
+            cache[key] = ops.pack_cols(self._sorted_v, n_src, row_bytes, budget_bytes=budget)
         return cache[key]
 
     def narrow_plan(self, n_src, row_bytes=64):
@@ -135,15 +136,20 @@ class EdgeIndex(object):
 
     def slot_scale(self, scale_src):
         """scale_src[cols[j]] for every CSR slot j -- the edge values of the normalised adjacency -- cached per scale
-        tensor (identity + in-place version counter), so the narrow-row kernel streams 4 bytes per slot instead of
-        gathering a 32-byte sector per edge."""
+        tensor (identity + in-place version counter), so the aggregation kernels stream 4 bytes per slot instead of
+        gathering a 32-byte sector per edge.  A scale is materialised on its second call in a row and None is
+        returned on the first: a one-off scale tensor (a fresh product in a backward pass) never pays an E-sized
+        build, a scale kept across calls (GCN's cached degree norm) hits from its second call on."""
         cache = self.__dict__.setdefault("_slot_scale_cache", {})
         key = (scale_src.data_ptr(), int(scale_src._version), int(scale_src.numel()))
-        hit = cache.get("key") == key
-        if not hit:
-            cache["key"] = key
-            cache["val"] = scale_src.reshape(-1)[self._sorted_v].contiguous()
-            cache["ref"] = scale_src          # keeps the storage alive, so the data_ptr cannot be recycled
+        if cache.get("key") == key:
+            return cache["val"]
+        if cache.get("seen") != key:
+            cache["seen"] = key
+            return None
+        cache["key"] = key
+        cache["val"] = scale_src.reshape(-1)[self._sorted_v].contiguous()
+        cache["ref"] = scale_src          # keeps the storage alive, so the data_ptr cannot be recycled
         return cache["val"]
 
     def csr(self):
