@@ -148,6 +148,25 @@ int pglb_spmm_csr_slot_scale_f32(const int64_t *indptr, const int64_t *cols, con
                                   another subset (halo rows) are still in flight */
 #define PGLB_SPMM_L2_HINTS 2   /* bit 31 of cols_packed carries an L2 residency hint */
 
+/* 16-bit feature types of pglb_spmm_csr_x16 */
+#define PGLB_DTYPE_BF16 1
+#define PGLB_DTYPE_F16 2
+/* Copy-message aggregation over 16-bit features: pglb_spmm_csr_slot_scale_f32 with msg_op = COPY (send_u_recv with
+ * every reduce_op; cols == NULL = identity slots, i.e. segment_*), where x and out are bfloat16 or float16 (`dtype`)
+ * and ldx / ldo count elements.  Numerics: every message is widened to fp32 exactly and reduced in fp32 in the same
+ * slot order and with the same operations as the fp32 entry; mean, scale_src / scale_slot / scale_dst (float32) and
+ * cut-row / hub partials (float32, in the workspace) stay fp32; each output element is rounded once, to nearest even.
+ * So every output equals round16(the fp32 entry's output on the widened x) whenever both take the same kernel: the
+ * wide-row kernel for copy sum / mean with 64 < D <= 128, D % 8 == 0, 16-byte aligned x and out and ldx, ldo % 8 == 0;
+ * the node-parallel kernel otherwise.
+ * ws: pglb_spmm_csr_ws(n_dst, E, D).  flags: PGLB_SPMM_L2_HINTS as above; PGLB_SPMM_ACCUMULATE is PGLB_EUNSUPPORTED
+ * (it would round twice).  Unknown dtype: PGLB_EINVAL.  All argument checks precede any CUDA call. */
+int pglb_spmm_csr_x16(const int64_t *indptr, const int64_t *cols, const void *x, int64_t ldx, void *out, int64_t ldo,
+                      int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t D, int dtype, int reduce_op,
+                      const float *scale_src, const float *scale_slot, const float *scale_dst,
+                      const uint32_t *cols_packed, int64_t max_degree_hint, int flags, void *ws, size_t ws_bytes,
+                      void *stream);
+
 /* Packed column ids for pglb_spmm_csr_f32: count[n_src] (int32, zeroed by the call) receives how
  * often every source occurs in cols[E]; packed[j] = cols[j] | (count[cols[j]] >= min_count) << 31.
  * Pass min_count = INT64_MAX for plain 32-bit ids without hints. */

@@ -13,6 +13,7 @@ PGLB_CUDA_ERR_BASE = 1000
 REDUCE = {"sum": 0, "mean": 1, "max": 2, "min": 3}
 MSG = {"copy": 0, "add": 1, "sub": 2, "mul": 3, "div": 4}
 BCAST_FULL, BCAST_HEAD, BCAST_SCALAR = 0, 1, 2
+DTYPE_BF16, DTYPE_F16 = 1, 2   # dtype of pglb_spmm_csr_x16
 
 
 class PglbError(RuntimeError):
@@ -50,6 +51,8 @@ _SIGS = {
     "pglb_spmm_csr_slot_scale_f32": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, c_int, _p, _i64, _i64, _i64, _i64,
                                              _i64, _i64, c_int, c_int, _p, _p, _p, _p, _i64, c_int, _p, c_size_t,
                                              _p]),
+    "pglb_spmm_csr_x16": (c_int, [_p, _p, _p, _i64, _p, _i64, _i64, _i64, _i64, _i64, c_int, c_int, _p, _p, _p, _p,
+                                  _i64, c_int, _p, c_size_t, _p]),
     "pglb_narrow_plan_ws": (c_int, [_i64, POINTER(c_size_t)]),
     "pglb_narrow_plan": (c_int, [_p, _p, _p, _i64, _i64, _i64, _p, _p, _p, _p, c_size_t, _p]),
     "pglb_spmm_narrow_ws": (c_int, [_i64, _i64, POINTER(c_size_t)]),

@@ -1,5 +1,7 @@
 // common.cuh -- shared helpers for libpglb (sm_90a only).
 #pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -77,5 +79,34 @@ int scan_i64(const int64_t *in, int64_t *out, int64_t n, int inclusive, void *tm
 // streaming (evict-first) loads for index data that is read exactly once
 __device__ __forceinline__ int64_t ld_stream(const int64_t *p) { return __ldcs((const long long *)p); }
 __device__ __forceinline__ int64_t ld_ro(const int64_t *p) { return __ldg((const long long *)p); }
+
+// 16-bit feature elements of pglb_spmm_csr_x16, handled as raw bits: widen() is exact, round() is the one
+// round-to-nearest-even of a value computed in fp32.  lo / hi = the element in the low / high half of a 32-bit word.
+template <typename T>
+struct X16;
+template <>
+struct X16<__nv_bfloat16> {
+    static __device__ __forceinline__ float widen(unsigned short b) { return __uint_as_float((unsigned)b << 16); }
+    static __device__ __forceinline__ float lo(unsigned w) { return __uint_as_float(w << 16); }
+    static __device__ __forceinline__ float hi(unsigned w) { return __uint_as_float(w & 0xffff0000u); }
+    static __device__ __forceinline__ unsigned short round(float f) { return __bfloat16_as_ushort(__float2bfloat16_rn(f)); }
+};
+template <>
+struct X16<__half> {
+    static __device__ __forceinline__ float widen(unsigned short b) { return __half2float(__ushort_as_half(b)); }
+    static __device__ __forceinline__ float lo(unsigned w) { return widen((unsigned short)(w & 0xffffu)); }
+    static __device__ __forceinline__ float hi(unsigned w) { return widen((unsigned short)(w >> 16)); }
+    static __device__ __forceinline__ unsigned short round(float f) { return __half_as_ushort(__float2half_rn(f)); }
+};
+// four consecutive 16-bit elements (8 bytes) <-> float4
+template <typename T>
+__device__ __forceinline__ float4 widen4(uint2 v) {
+    return make_float4(X16<T>::lo(v.x), X16<T>::hi(v.x), X16<T>::lo(v.y), X16<T>::hi(v.y));
+}
+template <typename T>
+__device__ __forceinline__ uint2 round4(float4 v) {
+    return make_uint2((unsigned)X16<T>::round(v.x) | ((unsigned)X16<T>::round(v.y) << 16),
+                      (unsigned)X16<T>::round(v.z) | ((unsigned)X16<T>::round(v.w) << 16));
+}
 
 }  // namespace pglb

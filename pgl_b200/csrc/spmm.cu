@@ -70,11 +70,29 @@ struct VecIO<4> {
     static __device__ __forceinline__ void st(float *p, const float (&v)[4]) {
         __stcs(reinterpret_cast<float4 *>(p), make_float4(v[0], v[1], v[2], v[3]));
     }
+    // 16-bit elements: 8 bytes per lane
+    template <typename T>
+    static __device__ __forceinline__ void ld(const T *p, float (&v)[4]) {
+        const float4 t = widen4<T>(__ldg(reinterpret_cast<const uint2 *>(p)));
+        v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+    }
+    template <typename T>
+    static __device__ __forceinline__ void st(T *p, const float (&v)[4]) {
+        __stcs(reinterpret_cast<uint2 *>(p), round4<T>(make_float4(v[0], v[1], v[2], v[3])));
+    }
 };
 template <>
 struct VecIO<1> {
     static __device__ __forceinline__ void ld(const float *p, float (&v)[1]) { v[0] = __ldg(p); }
     static __device__ __forceinline__ void st(float *p, const float (&v)[1]) { __stcs(p, v[0]); }
+    template <typename T>
+    static __device__ __forceinline__ void ld(const T *p, float (&v)[1]) {
+        v[0] = X16<T>::widen(__ldg(reinterpret_cast<const unsigned short *>(p)));
+    }
+    template <typename T>
+    static __device__ __forceinline__ void st(T *p, const float (&v)[1]) {
+        __stcs(reinterpret_cast<unsigned short *>(p), X16<T>::round(v[0]));
+    }
 };
 
 __device__ __forceinline__ float apply_msg(int op, float a, float b) {
@@ -89,8 +107,10 @@ __device__ __forceinline__ float apply_msg(int op, float a, float b) {
 
 // MODE 0: msg = x[col] (* scale_src);  MODE 1: msg = (x[col] (* scale_src)) op y[eid]
 // RK 0: sum / mean;  RK 1: max / min
-template <int VEC, int G, int ITERS, int MODE, int RK>
-__global__ void __launch_bounds__(kThreads) spmm_csr_kernel(const SpmmP p) {
+// TI / TO: element type of p.x / p.out (float, or the 16-bit type of pglb_spmm_csr_x16; its hub pass 1 writes fp32
+// partials and pass 2 reads them).  Messages are widened to fp32 on load, and each output is rounded once on store.
+template <typename TI, typename TO, int VEC, int G, int ITERS, int MODE, int RK>
+__device__ __forceinline__ void spmm_csr_body(const SpmmP &p) {
     constexpr int U = (8 / ITERS) < G ? (8 / ITERS) : G;
     const int lane = threadIdx.x & 31;
     const int gl = lane & (G - 1);
@@ -155,12 +175,12 @@ __global__ void __launch_bounds__(kThreads) spmm_csr_kernel(const SpmmP p) {
                 for (int j = 0; j < VEC; ++j) {
                     float a = acc[it][j];
                     if (deg == 0) a = 0.0f;
-                    if (p.accumulate) a = __fadd_rn(p.out[orow * p.ldo + col[it] + j], a);
+                    if (sizeof(TO) == 4 && p.accumulate) a = __fadd_rn(p.out[orow * p.ldo + col[it] + j], a);
                     if (p.reduce_op == PGLB_REDUCE_MEAN && deg != 0) a = __fdiv_rn(a, inv_cnt);
                     if (p.scale_dst) a = __fmul_rn(a, sd);
                     v[j] = a;
                 }
-                VecIO<VEC>::st(p.out + orow * p.ldo + col[it], v);
+                VecIO<VEC>::st(reinterpret_cast<TO *>(p.out) + orow * p.ldo + col[it], v);
             }
         };
 
@@ -193,7 +213,7 @@ __global__ void __launch_bounds__(kThreads) spmm_csr_kernel(const SpmmP p) {
                     int64_t e = 0;
                     if (MODE == 1) e = __shfl_sync(gmask, my_e, k0 + k, G);
                     if (k0 + k < nb) {
-                        const float *xr = p.x + c * p.ldx;
+                        const TI *xr = reinterpret_cast<const TI *>(p.x) + c * p.ldx;
 #pragma unroll
                         for (int it = 0; it < ITERS; ++it) {
                             if (act[it]) VecIO<VEC>::ld(xr + col[it], xv[k][it]);
@@ -255,6 +275,27 @@ __global__ void __launch_bounds__(kThreads) spmm_csr_kernel(const SpmmP p) {
             }
         }
     }
+}
+
+template <int VEC, int G, int ITERS, int MODE, int RK>
+__global__ void __launch_bounds__(kThreads) spmm_csr_kernel(const SpmmP p) {
+    spmm_csr_body<float, float, VEC, G, ITERS, MODE, RK>(p);
+}
+// copy messages over 16-bit features (pglb_spmm_csr_x16): TI / TO as above
+template <typename TI, typename TO, int VEC, int G, int ITERS, int RK>
+__global__ void __launch_bounds__(kThreads) spmm_csr_x16_kernel(const SpmmP p) {
+    spmm_csr_body<TI, TO, VEC, G, ITERS, 0, RK>(p);
+}
+// 4 elements per lane with 2 column iterations (129 <= D <= 256): under __launch_bounds__(kThreads)
+// ptxas holds these at 80 registers and spills 16-32 bytes; a cap of 96 registers instead removes the spills and ran
+// 11 % faster on an H100.  One element per lane (odd D, unaligned rows) also spills 8-24 bytes under the launch bound,
+// but capped it ran 17-26 % slower (more registers, fewer resident blocks), so it keeps the launch bound and its
+// spills, like the fp32 kernel of the same shape.
+template <int VEC, int ITERS>
+constexpr bool x16_capped() { return VEC == 4 && ITERS == 2; }
+template <typename TI, typename TO, int VEC, int G, int ITERS, int RK>
+__global__ void __maxnreg__(96) spmm_csr_x16_capped_kernel(const SpmmP p) {
+    spmm_csr_body<TI, TO, VEC, G, ITERS, 0, RK>(p);
 }
 
 // One block: turn the hub list into chunk tables.
@@ -373,6 +414,33 @@ static SpmmKernel pick_kernel(const Shape &s, int mode, int rk) {
     return s.vec == 4 ? pick_kernel_v<4>(s, mode, rk) : pick_kernel_v<1>(s, mode, rk);
 }
 
+template <typename TI, typename TO, int VEC, int G, int ITERS>
+static SpmmKernel pick_rk_x16(int rk) {
+    if constexpr (x16_capped<VEC, ITERS>())
+        return rk == 0 ? spmm_csr_x16_capped_kernel<TI, TO, VEC, G, ITERS, 0>
+                       : spmm_csr_x16_capped_kernel<TI, TO, VEC, G, ITERS, 1>;
+    else
+        return rk == 0 ? spmm_csr_x16_kernel<TI, TO, VEC, G, ITERS, 0> : spmm_csr_x16_kernel<TI, TO, VEC, G, ITERS, 1>;
+}
+
+template <typename TI, typename TO, int VEC>
+static SpmmKernel pick_kernel_x16_v(const Shape &s, int rk) {
+    switch (s.g) {
+        case 4: return pick_rk_x16<TI, TO, VEC, 4, 1>(rk);
+        case 8: return pick_rk_x16<TI, TO, VEC, 8, 1>(rk);
+        case 16: return pick_rk_x16<TI, TO, VEC, 16, 1>(rk);
+        default:
+            if (s.iters == 1) return pick_rk_x16<TI, TO, VEC, 32, 1>(rk);
+            if (s.iters == 2) return pick_rk_x16<TI, TO, VEC, 32, 2>(rk);
+            return pick_rk_x16<TI, TO, VEC, 32, 4>(rk);
+    }
+}
+
+template <typename TI, typename TO>
+static SpmmKernel pick_kernel_x16(const Shape &s, int rk) {
+    return s.vec == 4 ? pick_kernel_x16_v<TI, TO, 4>(s, rk) : pick_kernel_x16_v<TI, TO, 1>(s, rk);
+}
+
 struct HubWs {
     unsigned long long *hub_count;  // [1]
     int64_t *total_chunks;          // [1]
@@ -426,6 +494,14 @@ int gat_fused_run(const int64_t *indptr, const int64_t *cols, const float *f, in
                   const float *attn_src, const float *attn_dst, float slope, float *lse, void *ws, size_t ws_bytes,
                   cudaStream_t stream);
 
+// spmm_v5_kernel over 16-bit rows (copy sum / mean, 64 < D <= 128, D % 8 == 0): whether it takes a call, and the run
+bool stream_x16_eligible(const int64_t *cols, const uint32_t *cols32, const void *x, int64_t ldx, const void *out,
+                         int64_t ldo, int64_t n_src, int64_t E, int64_t D, int reduce_op);
+int spmm_stream_run_x16(int dtype, const int64_t *indptr, const int64_t *cols, const void *x, int64_t ldx, void *out,
+                        int64_t ldo, int64_t n_dst, int64_t E, int64_t D, int reduce_op,
+                        const float *scale_src, const float *scale_slot, const float *scale_dst, const uint32_t *cols32,
+                        int l2_hints, void *ws, size_t ws_bytes, cudaStream_t stream);
+
 bool stream_narrow_enabled();  // PGLB_NARROW=1: experimental narrow-row streaming kernel (spmm_stream.cu)
 
 static bool use_stream_path() {
@@ -435,6 +511,123 @@ static bool use_stream_path() {
         v = (e && strcmp(e, "legacy") == 0) ? 0 : 1;
     }
     return v == 1;
+}
+
+
+// The node-parallel launch sequence behind both entries: spmm_csr kernel over all rows, then, when some row is longer
+// than HUB_T slots, the hub plan and the two hub passes.  x / out are float, or 16-bit for pglb_spmm_csr_x16.
+// k_main runs over the rows, k_chunk turns hub chunks into fp32 partials, k_merge reduces a hub's partials into its row.
+static int spmm_generic_run(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const void *x,
+                            int64_t ldx, const float *y, int64_t ldy, int y_bcast, void *out, int64_t ldo,
+                            int64_t n_dst, int64_t num_edges, int64_t D, int64_t head_dim, int msg_op, int reduce_op,
+                            const float *scale_src, const float *scale_dst, int64_t max_degree_hint, int accumulate,
+                            const Shape &s, SpmmKernel k_main, SpmmKernel k_chunk, SpmmKernel k_merge, void *ws,
+                            size_t ws_bytes, cudaStream_t stream) {
+
+    const bool need_hub = !(max_degree_hint >= 0 && max_degree_hint <= HUB_T) && num_edges > HUB_T;
+    HubWs h{};
+    if (need_hub) {
+        h = layout_ws(ws, num_edges, D);
+        PGLB_CHECK_ARG(ws != nullptr && ws_bytes >= h.bytes, PGLB_EWORKSPACE,
+                       "pglb_spmm_csr: workspace of %zu bytes needed (got %zu)", h.bytes,
+                       ws_bytes);
+        PGLB_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
+                       "pglb_spmm_csr: workspace must be 256-byte aligned");
+        PGLB_CUDA(cudaMemsetAsync(h.hub_count, 0, 8, stream));
+    }
+
+    SpmmP p{};
+    p.rbeg = indptr;
+    p.rend = indptr + 1;
+    p.cols = cols;
+    p.eid = eid;
+    p.x = reinterpret_cast<const float *>(x);
+    p.ldx = ldx;
+    p.y = y;
+    p.ldy = ldy;
+    p.y_bcast = y_bcast;
+    p.out = reinterpret_cast<float *>(out);
+    p.ldo = ldo;
+    p.n_rows = n_dst;
+    p.n_rows_dev = nullptr;
+    p.D = (int)D;
+    p.head_dim = (int)(head_dim > 0 ? head_dim : 1);
+    p.msg_op = msg_op;
+    p.reduce_op = reduce_op;
+    p.scale_src = scale_src;
+    p.scale_dst = scale_dst;
+    p.row_map = nullptr;
+    p.mean_indptr = nullptr;
+    p.rpg = 8;
+    p.contig = 1;
+    p.hub_threshold = need_hub ? HUB_T : INT64_MAX;
+    p.hub_count = h.hub_count;
+    p.hub_rows = h.hub_rows;
+    p.accumulate = accumulate;
+
+    const int64_t gpb = kThreads / s.g;
+    {
+        const int64_t tasks = (n_dst + p.rpg - 1) / p.rpg;
+        const int64_t blocks = (tasks + gpb - 1) / gpb;
+        PGLB_CHECK_ARG(blocks <= 0x7fffffffLL, PGLB_ESHAPE, "pglb_spmm_csr: grid too large");
+        dim3 grid((unsigned)blocks, (unsigned)s.tiles);
+        k_main<<<grid, kThreads, 0, stream>>>(p);
+        PGLB_LAUNCH_CHECK("spmm_csr_kernel");
+    }
+    if (need_hub) {
+        hub_plan_kernel<<<1, 1024, 0, stream>>>(indptr, h.hub_count, h.hub_rows, h.chunk_off,
+                                                h.vbeg, h.vend, h.total_chunks, h.n_hubs);
+        PGLB_LAUNCH_CHECK("hub_plan_kernel");
+        const int64_t max_blocks = (int64_t)sm_count() * 8;
+        // pass 1: chunk -> partial (same message, SUM/MAX/MIN, no row epilogue)
+        SpmmP p1 = p;
+        p1.rbeg = h.vbeg;
+        p1.rend = h.vend;
+        p1.out = h.partial;
+        p1.ldo = h.dpad;
+        p1.n_rows = 0;
+        p1.n_rows_dev = h.total_chunks;
+        p1.reduce_op = (reduce_op == PGLB_REDUCE_MEAN) ? PGLB_REDUCE_SUM : reduce_op;
+        p1.scale_dst = nullptr;
+        p1.rpg = 1;
+        p1.contig = 0;
+        p1.accumulate = 0;
+        p1.hub_threshold = INT64_MAX;
+        {
+            int64_t blocks = (h.chunk_cap + gpb - 1) / gpb;
+            if (blocks > max_blocks) blocks = max_blocks;
+            // partial rows are dpad floats, 16-byte aligned => same vector shape is valid
+            dim3 grid((unsigned)blocks, (unsigned)s.tiles);
+            k_chunk<<<grid, kThreads, 0, stream>>>(p1);
+            PGLB_LAUNCH_CHECK("spmm_csr_kernel(hub pass 1)");
+        }
+        // pass 2: partials of a hub -> its output row
+        SpmmP p2 = p;
+        p2.rbeg = h.chunk_off;
+        p2.rend = h.chunk_off + 1;
+        p2.cols = nullptr;
+        p2.eid = nullptr;
+        p2.x = h.partial;
+        p2.ldx = h.dpad;
+        p2.y = nullptr;
+        p2.msg_op = PGLB_MSG_COPY;
+        p2.scale_src = nullptr;
+        p2.n_rows = 0;
+        p2.n_rows_dev = h.n_hubs;
+        p2.row_map = h.hub_rows;
+        p2.mean_indptr = indptr;
+        p2.rpg = 1;
+        p2.contig = 0;
+        p2.hub_threshold = INT64_MAX;
+        {
+            int64_t blocks = (h.hub_cap + gpb - 1) / gpb;
+            if (blocks > max_blocks) blocks = max_blocks;
+            dim3 grid((unsigned)blocks, (unsigned)s.tiles);
+            k_merge<<<grid, kThreads, 0, stream>>>(p2);
+            PGLB_LAUNCH_CHECK("spmm_csr_kernel(hub pass 2)");
+        }
+    }
+    return PGLB_OK;
 }
 
 }  // namespace pglb
@@ -518,111 +711,54 @@ extern "C" int pglb_spmm_csr_slot_scale_f32(const int64_t *indptr, const int64_t
     }
     const Shape s = pick_shape(D, vec4);
     const int rk = (reduce_op >= PGLB_REDUCE_MAX) ? 1 : 0;
+    return spmm_generic_run(indptr, cols, eid, x, ldx, y, ldy, y_bcast, out, ldo, n_dst, num_edges, D, head_dim, msg_op,
+                            reduce_op, scale_src, scale_dst, max_degree_hint, accumulate, s, pick_kernel(s, mode, rk),
+                            pick_kernel(s, mode, rk), pick_kernel(s, 0, rk), ws, ws_bytes, stream);
+}
 
-    const bool need_hub = !(max_degree_hint >= 0 && max_degree_hint <= HUB_T) && num_edges > HUB_T;
-    HubWs h{};
-    if (need_hub) {
-        h = layout_ws(ws, num_edges, D);
-        PGLB_CHECK_ARG(ws != nullptr && ws_bytes >= h.bytes, PGLB_EWORKSPACE,
-                       "pglb_spmm_csr_f32: workspace of %zu bytes needed (got %zu)", h.bytes,
-                       ws_bytes);
+extern "C" int pglb_spmm_csr_x16(const int64_t *indptr, const int64_t *cols, const void *x, int64_t ldx, void *out,
+                                 int64_t ldo, int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t D, int dtype,
+                                 int reduce_op, const float *scale_src, const float *scale_slot,
+                                 const float *scale_dst, const uint32_t *cols_packed, int64_t max_degree_hint,
+                                 int flags, void *ws, size_t ws_bytes, void *stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL,
+                   "pglb_spmm_csr_x16: unknown dtype %d", dtype);
+    PGLB_CHECK_ARG(n_dst >= 0 && n_src >= 0 && num_edges >= 0 && D >= 0, PGLB_EINVAL,
+                   "pglb_spmm_csr_x16: negative size");
+    PGLB_CHECK_ARG(reduce_op >= PGLB_REDUCE_SUM && reduce_op <= PGLB_REDUCE_MIN, PGLB_EINVAL,
+                   "pglb_spmm_csr_x16: unknown reduce_op %d", reduce_op);
+    PGLB_CHECK_ARG(!scale_slot || scale_src, PGLB_EINVAL, "pglb_spmm_csr_x16: scale_slot needs scale_src");
+    PGLB_CHECK_ARG(!(flags & PGLB_SPMM_ACCUMULATE), PGLB_EUNSUPPORTED,
+                   "pglb_spmm_csr_x16: PGLB_SPMM_ACCUMULATE would round the output twice");
+    if (n_dst == 0 || D == 0) return PGLB_OK;
+    PGLB_CHECK_ARG(indptr && out, PGLB_EINVAL, "pglb_spmm_csr_x16: indptr/out is NULL");
+    PGLB_CHECK_ARG(num_edges == 0 || x, PGLB_EINVAL, "pglb_spmm_csr_x16: x is NULL");
+    PGLB_CHECK_ARG(ldx >= D && ldo >= D, PGLB_ESHAPE, "pglb_spmm_csr_x16: leading dimension smaller than D");
+    PGLB_CHECK_ARG(D <= INT32_MAX, PGLB_ESHAPE, "pglb_spmm_csr_x16: D too large");
+    if (num_edges > 0 && use_stream_path() &&
+        stream_x16_eligible(cols, cols_packed, x, ldx, out, ldo, n_src, num_edges, D, reduce_op)) {
         PGLB_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
-                       "pglb_spmm_csr_f32: workspace must be 256-byte aligned");
-        PGLB_CUDA(cudaMemsetAsync(h.hub_count, 0, 8, stream));
+                       "pglb_spmm_csr_x16: workspace must be 256-byte aligned");
+        return spmm_stream_run_x16(dtype, indptr, cols, x, ldx, out, ldo, n_dst, num_edges, D, reduce_op,
+                                   scale_src, scale_slot, scale_dst, cols_packed,
+                                   (flags & PGLB_SPMM_L2_HINTS) ? 1 : 0, ws, ws_bytes, stream);
     }
-
-    SpmmP p{};
-    p.rbeg = indptr;
-    p.rend = indptr + 1;
-    p.cols = cols;
-    p.eid = eid;
-    p.x = x;
-    p.ldx = ldx;
-    p.y = y;
-    p.ldy = ldy;
-    p.y_bcast = y_bcast;
-    p.out = out;
-    p.ldo = ldo;
-    p.n_rows = n_dst;
-    p.n_rows_dev = nullptr;
-    p.D = (int)D;
-    p.head_dim = (int)(head_dim > 0 ? head_dim : 1);
-    p.msg_op = msg_op;
-    p.reduce_op = reduce_op;
-    p.scale_src = scale_src;
-    p.scale_dst = scale_dst;
-    p.row_map = nullptr;
-    p.mean_indptr = nullptr;
-    p.rpg = 8;
-    p.contig = 1;
-    p.hub_threshold = need_hub ? HUB_T : INT64_MAX;
-    p.hub_count = h.hub_count;
-    p.hub_rows = h.hub_rows;
-    p.accumulate = accumulate;
-
-    const int64_t gpb = kThreads / s.g;
-    {
-        const int64_t tasks = (n_dst + p.rpg - 1) / p.rpg;
-        const int64_t blocks = (tasks + gpb - 1) / gpb;
-        PGLB_CHECK_ARG(blocks <= 0x7fffffffLL, PGLB_ESHAPE, "pglb_spmm_csr_f32: grid too large");
-        dim3 grid((unsigned)blocks, (unsigned)s.tiles);
-        pick_kernel(s, mode, rk)<<<grid, kThreads, 0, stream>>>(p);
-        PGLB_LAUNCH_CHECK("spmm_csr_kernel");
-    }
-    if (need_hub) {
-        hub_plan_kernel<<<1, 1024, 0, stream>>>(indptr, h.hub_count, h.hub_rows, h.chunk_off,
-                                                h.vbeg, h.vend, h.total_chunks, h.n_hubs);
-        PGLB_LAUNCH_CHECK("hub_plan_kernel");
-        const int64_t max_blocks = (int64_t)sm_count() * 8;
-        // pass 1: chunk -> partial (same message, SUM/MAX/MIN, no row epilogue)
-        SpmmP p1 = p;
-        p1.rbeg = h.vbeg;
-        p1.rend = h.vend;
-        p1.out = h.partial;
-        p1.ldo = h.dpad;
-        p1.n_rows = 0;
-        p1.n_rows_dev = h.total_chunks;
-        p1.reduce_op = (reduce_op == PGLB_REDUCE_MEAN) ? PGLB_REDUCE_SUM : reduce_op;
-        p1.scale_dst = nullptr;
-        p1.rpg = 1;
-        p1.contig = 0;
-        p1.accumulate = 0;
-        p1.hub_threshold = INT64_MAX;
-        {
-            int64_t blocks = (h.chunk_cap + gpb - 1) / gpb;
-            if (blocks > max_blocks) blocks = max_blocks;
-            // partial rows are dpad floats, 16-byte aligned => same vector shape is valid
-            dim3 grid((unsigned)blocks, (unsigned)s.tiles);
-            pick_kernel(s, mode, rk)<<<grid, kThreads, 0, stream>>>(p1);
-            PGLB_LAUNCH_CHECK("spmm_csr_kernel(hub pass 1)");
-        }
-        // pass 2: partials of a hub -> its output row
-        SpmmP p2 = p;
-        p2.rbeg = h.chunk_off;
-        p2.rend = h.chunk_off + 1;
-        p2.cols = nullptr;
-        p2.eid = nullptr;
-        p2.x = h.partial;
-        p2.ldx = h.dpad;
-        p2.y = nullptr;
-        p2.msg_op = PGLB_MSG_COPY;
-        p2.scale_src = nullptr;
-        p2.n_rows = 0;
-        p2.n_rows_dev = h.n_hubs;
-        p2.row_map = h.hub_rows;
-        p2.mean_indptr = indptr;
-        p2.rpg = 1;
-        p2.contig = 0;
-        p2.hub_threshold = INT64_MAX;
-        {
-            int64_t blocks = (h.hub_cap + gpb - 1) / gpb;
-            if (blocks > max_blocks) blocks = max_blocks;
-            dim3 grid((unsigned)blocks, (unsigned)s.tiles);
-            pick_kernel(s, 0, rk)<<<grid, kThreads, 0, stream>>>(p2);
-            PGLB_LAUNCH_CHECK("spmm_csr_kernel(hub pass 2)");
-        }
-    }
-    return PGLB_OK;
+    // every other shape: the node-parallel kernel, 8 bytes (4 elements) per lane when rows allow it
+    auto aligned8 = [](const void *q) { return (reinterpret_cast<uintptr_t>(q) & 7u) == 0; };
+    const bool vec4 = (D % 4 == 0) && (ldx % 4 == 0) && (ldo % 4 == 0) && aligned8(x) && aligned8(out);
+    const Shape s = pick_shape(D, vec4);
+    const int rk = (reduce_op >= PGLB_REDUCE_MAX) ? 1 : 0;
+    if (dtype == PGLB_DTYPE_BF16)
+        return spmm_generic_run(indptr, cols, nullptr, x, ldx, nullptr, 0, 0, out, ldo, n_dst, num_edges, D, 1,
+                                PGLB_MSG_COPY, reduce_op, scale_src, scale_dst, max_degree_hint, 0, s,
+                                pick_kernel_x16<__nv_bfloat16, __nv_bfloat16>(s, rk),
+                                pick_kernel_x16<__nv_bfloat16, float>(s, rk),
+                                pick_kernel_x16<float, __nv_bfloat16>(s, rk), ws, ws_bytes, stream);
+    return spmm_generic_run(indptr, cols, nullptr, x, ldx, nullptr, 0, 0, out, ldo, n_dst, num_edges, D, 1,
+                            PGLB_MSG_COPY, reduce_op, scale_src, scale_dst, max_degree_hint, 0, s,
+                            pick_kernel_x16<__half, __half>(s, rk), pick_kernel_x16<__half, float>(s, rk),
+                            pick_kernel_x16<float, __half>(s, rk), ws, ws_bytes, stream);
 }
 
 static int gat_fused_entry(const char *name, const int64_t *indptr, const int64_t *cols, const float *f, int64_t ldf,

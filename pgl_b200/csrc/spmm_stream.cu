@@ -36,7 +36,7 @@ constexpr int SW = 7;     // warps per block (7 * 16 KB = 112 KB smem, two block
 struct StreamP {
     const int64_t *indptr;
     const int64_t *cols;  // nullable: identity
-    const float *x;
+    const float *x;  // x / out: float, or the 16-bit element type of the *_x16 kernels (ldx / ldo in elements)
     int64_t ldx;
     float *out;
     int64_t ldo;
@@ -696,9 +696,10 @@ __global__ void __launch_bounds__(StreamCfg<ITERS>::kThreads) spmm_stream_kernel
     if (lane == 0 && blockIdx.y == 0) p.tail_row[task] = tail;
 }
 
-// One warp per task that owns a cut row: out[r] = epilogue(tail(t) (+) head(t+1) (+) ...)
-template <int ITERS, int RK>
-__global__ void __launch_bounds__(256) spmm_stream_fixup_kernel(const StreamP p) {
+// One warp per task that owns a cut row: out[r] = epilogue(tail(t) (+) head(t+1) (+) ...).  The partials are fp32;
+// TO is the element type of out (a 16-bit out is rounded once, on the store).
+template <typename TO, int ITERS, int RK>
+__device__ __forceinline__ void spmm_stream_fixup_body(const StreamP &p) {
     const int lane = threadIdx.x & 31;
     const int64_t t = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (t >= p.ntasks) return;
@@ -738,7 +739,7 @@ __global__ void __launch_bounds__(256) spmm_stream_fixup_kernel(const StreamP p)
         }
         for (; u < u_end; ++u)
             comb(*reinterpret_cast<const float4 *>(p.partial + (2 * u) * p.dpad + c));
-        if (p.accumulate) {
+        if (sizeof(TO) == 4 && p.accumulate) {
             const float4 o = *reinterpret_cast<const float4 *>(p.out + r * p.ldo + c);
             acc.x = __fadd_rn(o.x, acc.x); acc.y = __fadd_rn(o.y, acc.y);
             acc.z = __fadd_rn(o.z, acc.z); acc.w = __fadd_rn(o.w, acc.w);
@@ -753,8 +754,20 @@ __global__ void __launch_bounds__(256) spmm_stream_fixup_kernel(const StreamP p)
             acc.x = __fmul_rn(acc.x, sd); acc.y = __fmul_rn(acc.y, sd);
             acc.z = __fmul_rn(acc.z, sd); acc.w = __fmul_rn(acc.w, sd);
         }
-        *reinterpret_cast<float4 *>(p.out + r * p.ldo + c) = acc;
+        if constexpr (sizeof(TO) == 4)
+            *reinterpret_cast<float4 *>(p.out + r * p.ldo + c) = acc;
+        else
+            *reinterpret_cast<uint2 *>(reinterpret_cast<TO *>(p.out) + r * p.ldo + c) = round4<TO>(acc);
     }
+}
+
+template <int ITERS, int RK>
+__global__ void __launch_bounds__(256) spmm_stream_fixup_kernel(const StreamP p) {
+    spmm_stream_fixup_body<float, ITERS, RK>(p);
+}
+template <typename T>
+__global__ void __launch_bounds__(256) spmm_stream_fixup_x16_kernel(const StreamP p) {
+    spmm_stream_fixup_body<T, 1, 0>(p);
 }
 
 // Fused-GAT fix-up: merge the (acc, m, l) partials of a cut row: M = max m_i,
@@ -789,11 +802,12 @@ __global__ void __launch_bounds__(256) spmm_stream_fixup_gat_kernel(const Stream
 }
 
 // Rows without a slot: zero (or, when accumulating, out_prev * scale_dst).  One warp looks at 32
-// rows at a time; the streaming tasks above never touch empty rows.
-__global__ void __launch_bounds__(256) empty_rows_kernel(const int64_t *__restrict__ indptr,
-                                                         int64_t n_rows, int D, float *__restrict__ out,
-                                                         int64_t ldo, const float *__restrict__ scale_dst,
-                                                         int accumulate) {
+// rows at a time; the streaming tasks above never touch empty rows.  TO: element type of out (16-bit: D % 4 == 0,
+// rows 8-byte aligned, never accumulating).
+template <typename TO>
+__device__ __forceinline__ void empty_rows_body(const int64_t *__restrict__ indptr, int64_t n_rows, int D,
+                                                float *__restrict__ out, int64_t ldo,
+                                                const float *__restrict__ scale_dst, int accumulate) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -807,6 +821,10 @@ __global__ void __launch_bounds__(256) empty_rows_kernel(const int64_t *__restri
             mask &= mask - 1;
             float *row = out + (r0 + i) * ldo;
             for (int c = lane * 4; c < D; c += 128) {
+                if constexpr (sizeof(TO) == 2) {
+                    *reinterpret_cast<uint2 *>(reinterpret_cast<TO *>(out) + (r0 + i) * ldo + c) = make_uint2(0u, 0u);
+                    continue;
+                }
                 float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
                 if (accumulate) {
                     v = *reinterpret_cast<const float4 *>(row + c);
@@ -819,6 +837,18 @@ __global__ void __launch_bounds__(256) empty_rows_kernel(const int64_t *__restri
             }
         }
     }
+}
+
+__global__ void __launch_bounds__(256) empty_rows_kernel(const int64_t *__restrict__ indptr,
+                                                         int64_t n_rows, int D, float *__restrict__ out,
+                                                         int64_t ldo, const float *__restrict__ scale_dst,
+                                                         int accumulate) {
+    empty_rows_body<float>(indptr, n_rows, D, out, ldo, scale_dst, accumulate);
+}
+template <typename T>
+__global__ void __launch_bounds__(256) empty_rows_x16_kernel(const int64_t *__restrict__ indptr, int64_t n_rows, int D,
+                                                             float *__restrict__ out, int64_t ldo) {
+    empty_rows_body<T>(indptr, n_rows, D, out, ldo, nullptr, 0);
 }
 
 static int launch_empty_rows(const StreamP &p, cudaStream_t stream) {
@@ -1235,24 +1265,22 @@ static int launch_stream(const StreamP &p, int tiles, cudaStream_t stream) {
     return PGLB_OK;
 }
 
-// Called by pglb_spmm_csr_f32 for the eligible shapes.  `ws` holds >= stream_ws_bytes().
-int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, int64_t ldx,
-                    float *out, int64_t ldo, int64_t n_dst, int64_t n_src, int64_t E, int64_t D,
-                    int reduce_op, const float *scale_src, const float *scale_slot, const float *scale_dst,
-                    const uint32_t *cols32, int l2_hints, int accumulate, const int64_t *eid,
-                    const float *y, int64_t ldy, int y_bcast, int head_dim, int msg_op, void *ws,
-                    size_t ws_bytes, cudaStream_t stream) {
+// Task plan and launch parameters shared by the wide-row runs below; fills everything of p but the edge operand and
+// accumulate (left as the caller set them).  `ws` holds >= stream_ws_bytes().
+static int stream_prepare(StreamP &p, const int64_t *indptr, const int64_t *cols, const void *x, int64_t ldx,
+                          void *out, int64_t ldo, int64_t n_dst, int64_t E, int64_t D, int reduce_op,
+                          const float *scale_src, const float *scale_slot, const float *scale_dst,
+                          const uint32_t *cols32, void *ws, size_t ws_bytes, cudaStream_t stream) {
     const int64_t T = stream_task_size(E);
     PGLB_CHECK_ARG(E > 0, PGLB_EINVAL, "spmm_stream_run: needs at least one slot");
     StreamWs w = stream_layout(ws, E, D, T);
     PGLB_CHECK_ARG(ws != nullptr && ws_bytes >= w.bytes, PGLB_EWORKSPACE,
-                   "pglb_spmm_csr_f32: workspace of %zu bytes needed (got %zu)", w.bytes, ws_bytes);
-    StreamP p{};
+                   "pglb_spmm_csr: workspace of %zu bytes needed (got %zu)", w.bytes, ws_bytes);
     p.indptr = indptr;
     p.cols = cols;
-    p.x = x;
+    p.x = reinterpret_cast<const float *>(x);
     p.ldx = ldx;
-    p.out = out;
+    p.out = reinterpret_cast<float *>(out);
     p.ldo = ldo;
     p.n_rows = n_dst;
     p.E = E;
@@ -1269,13 +1297,6 @@ int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, 
     p.dpad = w.dpad;
     p.tail_row = w.tail_row;
     p.cols32 = cols32;
-    p.eid = eid;
-    p.y = y;
-    p.ldy = ldy;
-    p.y_bcast = y_bcast;
-    p.head_dim = head_dim > 0 ? head_dim : 1;
-    p.msg_op = msg_op;
-    p.accumulate = accumulate;
     {
         static int mode = 0;
         if (mode == 0) {
@@ -1294,6 +1315,29 @@ int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, 
                                                                w.ntasks, w.first_row, w.start, w.counter);
         PGLB_LAUNCH_CHECK("task_plan_kernel");
     }
+    return PGLB_OK;
+}
+
+// Called by pglb_spmm_csr_f32 for the eligible shapes.  `ws` holds >= stream_ws_bytes().
+int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, int64_t ldx,
+                    float *out, int64_t ldo, int64_t n_dst, int64_t n_src, int64_t E, int64_t D,
+                    int reduce_op, const float *scale_src, const float *scale_slot, const float *scale_dst,
+                    const uint32_t *cols32, int l2_hints, int accumulate, const int64_t *eid,
+                    const float *y, int64_t ldy, int y_bcast, int head_dim, int msg_op, void *ws,
+                    size_t ws_bytes, cudaStream_t stream) {
+    StreamP p{};
+    p.eid = eid;
+    p.y = y;
+    p.ldy = ldy;
+    p.y_bcast = y_bcast;
+    p.head_dim = head_dim > 0 ? head_dim : 1;
+    p.msg_op = msg_op;
+    p.accumulate = accumulate;
+    {
+        const int rc = stream_prepare(p, indptr, cols, x, ldx, out, ldo, n_dst, E, D, reduce_op, scale_src, scale_slot,
+                                      scale_dst, cols32, ws, ws_bytes, stream);
+        if (rc) return rc;
+    }
     {
         const int rc = launch_empty_rows(p, stream);
         if (rc) return rc;
@@ -1310,7 +1354,7 @@ int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, 
     }
     if (cv <= 32 && v5_eligible(p, n_src, rk, small_ids))
         return launch_v5(p, cols32 != nullptr && cols != nullptr && l2_hints != 0, stream);
-    p.dyn = dyn_mode("PGLB_S128_DYN", 2, w.ntasks);   // round 1's kernel (max / min, edge operands): descending queue
+    p.dyn = dyn_mode("PGLB_S128_DYN", 2, p.ntasks);   // round 1's kernel (max / min, edge operands): descending queue
     if (cv <= 32 && small_ids) {
         if (y) {  // edge operand: plain int64 ids, no source scale
             return rk ? launch_stream128<1, false, 0, 1>(p, stream) : launch_stream128<0, false, 0, 1>(p, stream);
@@ -1327,6 +1371,44 @@ int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, 
     const int tiles = (int)((cv + 32 * iters - 1) / (32 * iters));
     if (iters == 2) return rk ? launch_stream<2, 1>(p, tiles, stream) : launch_stream<2, 0>(p, tiles, stream);
     return rk ? launch_stream<4, 1>(p, tiles, stream) : launch_stream<4, 0>(p, tiles, stream);
+}
+
+// spmm_v5_kernel over 16-bit rows: copy sum / mean, 64 < D <= 128, rows a multiple of 16 bytes (D % 8 == 0, as a bulk
+// copy needs), 16-byte aligned x and out, ids that fit the packed form.  Every other 16-bit call takes the node-parallel
+// kernel (spmm.cu).
+bool stream_x16_eligible(const int64_t *cols, const uint32_t *cols32, const void *x, int64_t ldx, const void *out,
+                         int64_t ldo, int64_t n_src, int64_t E, int64_t D, int reduce_op) {
+    if (v5_mode() == 0 || reduce_op >= PGLB_REDUCE_MAX || D <= 64 || D > 128 || D % 8 != 0) return false;
+    if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(out) & 15) || ldx % 8 || ldo % 8)
+        return false;
+    if ((cols ? n_src : E) >= 0x7fffffffLL || ldx * 2 >= 0xffffffffLL) return false;  // small_ids of the fp32 run
+    if (v5_mode() == 1 && (n_src >= 0x7fffffffLL || (!cols && !cols32))) return false;  // as v5_eligible
+    return true;
+}
+
+template <typename T>
+static int run_x16(const StreamP &p, bool hot, cudaStream_t stream) {
+    int64_t blocks = (p.n_rows + 255) / 256;
+    const int64_t cap = (int64_t)sm_count() * 8;
+    if (blocks > cap) blocks = cap;
+    if (blocks < 1) blocks = 1;
+    empty_rows_x16_kernel<T><<<(unsigned)blocks, 256, 0, stream>>>(p.indptr, p.n_rows, p.D, p.out, p.ldo);
+    PGLB_LAUNCH_CHECK("empty_rows_kernel");
+    return launch_v5<T>(p, hot, stream);
+}
+
+// Called by pglb_spmm_csr_x16 when stream_x16_eligible().  `ws` holds >= stream_ws_bytes().
+int spmm_stream_run_x16(int dtype, const int64_t *indptr, const int64_t *cols, const void *x, int64_t ldx, void *out,
+                        int64_t ldo, int64_t n_dst, int64_t E, int64_t D, int reduce_op,
+                        const float *scale_src, const float *scale_slot, const float *scale_dst, const uint32_t *cols32,
+                        int l2_hints, void *ws, size_t ws_bytes, cudaStream_t stream) {
+    StreamP p{};
+    p.head_dim = 1;
+    const int rc = stream_prepare(p, indptr, cols, x, ldx, out, ldo, n_dst, E, D, reduce_op, scale_src, scale_slot,
+                                  scale_dst, cols32, ws, ws_bytes, stream);
+    if (rc) return rc;
+    const bool hot = cols32 != nullptr && cols != nullptr && l2_hints != 0;
+    return dtype == PGLB_DTYPE_BF16 ? run_x16<__nv_bfloat16>(p, hot, stream) : run_x16<__half>(p, hot, stream);
 }
 
 

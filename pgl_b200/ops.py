@@ -49,55 +49,83 @@ def _i64(t):
     return t
 
 
-def f64_through(fn):
-    """float64 in -> float64 out for the public feature ops (the reference's tests/test_conv.py:43-71 runs GCN,
-    GraphSage and GAT in float64).  The kernels are fp32: float64 tensors are rounded to float32 on the way in and
-    the result is widened on the way out (autograd flows through both casts), so a float64 caller gets fp32-accurate
-    values in its own dtype -- within the path's stated 1e-4 relative tolerance, not fp64 accuracy (INTEGRATION.md)."""
-    import functools
+HALF_DTYPES = (torch.bfloat16, torch.float16)
+_DTYPE16 = {torch.bfloat16: _lib.DTYPE_BF16, torch.float16: _lib.DTYPE_F16}
 
-    def is64(t):
-        return isinstance(t, torch.Tensor) and t.dtype == torch.float64
 
-    def down(v):
-        mat = getattr(v, "materialize", None)
-        if mat is not None and getattr(v, "dtype", None) == torch.float64:
-            v = mat()
-        if is64(v):
-            return v.to(torch.float32)
+def _cast_through(fn, native16):
+    """Run fp32 kernels for callers in other float dtypes; autograd flows through every cast.
+    float64 anywhere in the arguments: every float64 and 16-bit tensor is rounded / widened to float32 on the way in
+    and the float32 results are widened to float64 on the way out.  Otherwise, unless `native16` (fn has 16-bit kernels
+    of its own and takes such tensors as they are), 16-bit tensors are widened to float32 exactly, the fp32 kernels
+    run, and float32 results are rounded to the promoted dtype of the floating-point tensor arguments (torch
+    promotion: bf16 with fp32 gives fp32)."""
+
+    def dtype_of(v):
+        return v.dtype if isinstance(v, torch.Tensor) or hasattr(v, "materialize") else None
+
+    def dtypes(v):
+        d = dtype_of(v)
+        if d is not None:
+            return [d] if d.is_floating_point else []
         if isinstance(v, (list, tuple)):
-            return type(v)(down(a) for a in v)
+            return [x for a in v for x in dtypes(a)]
+        return []
+
+    def to32(v, widen):
+        if dtype_of(v) in widen:
+            mat = getattr(v, "materialize", None)
+            return (mat() if mat is not None else v).to(torch.float32)
+        if isinstance(v, (list, tuple)):
+            return type(v)(to32(a, widen) for a in v)
         return v
 
-    def any64(v):
-        if is64(v) or (hasattr(v, "materialize") and getattr(v, "dtype", None) == torch.float64):
-            return True
-        return isinstance(v, (list, tuple)) and any(any64(a) for a in v)
-
-    def up(v):
+    def back(v, dtype):
         if isinstance(v, torch.Tensor) and v.dtype == torch.float32:
-            return v.to(torch.float64)
+            return v.to(dtype)
         if isinstance(v, tuple):
-            return tuple(up(a) for a in v)
+            return tuple(back(a, dtype) for a in v)
         return v
 
     @functools.wraps(fn)
     def wrapper(*args, **kwargs):
-        if not (any(any64(a) for a in args) or any(any64(a) for a in kwargs.values())):
+        found = [d for a in list(args) + list(kwargs.values()) for d in dtypes(a)]
+        if torch.float64 in found:
+            widen, result = (torch.float64,) + HALF_DTYPES, torch.float64
+        elif not native16 and any(d in HALF_DTYPES for d in found):
+            widen, result = HALF_DTYPES, functools.reduce(torch.promote_types, found)
+        else:
             return fn(*args, **kwargs)
-        out = fn(*[down(a) for a in args], **{k: down(a) for k, a in kwargs.items()})
-        return up(out)
+        out = fn(*[to32(a, widen) for a in args], **{k: to32(a, widen) for k, a in kwargs.items()})
+        return back(out, result) if result != torch.float32 else out
     return wrapper
 
 
-def _f32_2d(t):
+def f64_through(fn):
+    """float64 in -> float64 out for the public feature ops (the reference's tests/test_conv.py:43-71 runs GCN,
+    GraphSage and GAT in float64), and bfloat16 / float16 in -> the same dtype out for ops without 16-bit kernels.
+    The kernels are fp32: float64 tensors are rounded to float32 on the way in and the result is widened on the way
+    out, so a float64 caller gets fp32-accurate values in its own dtype -- within the path's stated 1e-4 relative
+    tolerance, not fp64 accuracy (INTEGRATION.md).  16-bit tensors are widened exactly and the result rounded once
+    (see _cast_through)."""
+    return _cast_through(fn, native16=False)
+
+
+def native16_through(fn):
+    """f64_through for the ops with 16-bit kernels of their own (copy aggregation, segment_*): bfloat16 / float16
+    features reach them unchanged; float64 follows f64_through."""
+    return _cast_through(fn, native16=True)
+
+
+def _f32_2d(t, allow16=False):
     """[n, d1, d2, ...] -> contiguous [n, D] float32 view (no copy when already so).  A lazy row
     gather (utils.op.LazyRows) is resolved to its plain tensor first: the wrapper itself carries no
-    autograd state, so requires_grad must be read from the gathered result."""
+    autograd state, so requires_grad must be read from the gathered result.  allow16: bfloat16 / float16 pass
+    too (the copy aggregation's 16-bit route)."""
     mat = getattr(t, "materialize", None)
     if mat is not None:
         t = mat()
-    if t.dtype != torch.float32:
+    if t.dtype != torch.float32 and not (allow16 and t.dtype in HALF_DTYPES):
         raise TypeError("pgl_b200: float32 features expected on the CUDA path, got %s" % t.dtype)
     t2 = t.reshape(t.shape[0], -1) if t.dim() != 2 else t
     if not t2.is_contiguous():
@@ -264,6 +292,14 @@ def _spmm_raw(indptr, cols, x2, n_dst, reduce_op, eid=None, y2=None, y_bcast=BCA
     dev = x2.device
     D = int(x2.shape[1])
     E = int(num_edges if num_edges is not None else (cols.shape[0] if cols is not None else 0))
+    # the norms are fp32 on every route (an N-sized cast for a 16-bit norm)
+    if scale_src is not None and scale_src.dtype != torch.float32:
+        scale_src = scale_src.float()
+    if scale_dst is not None and scale_dst.dtype != torch.float32:
+        scale_dst = scale_dst.float()
+    if x2.dtype in HALF_DTYPES:
+        return _spmm_x16(indptr, cols, x2, n_dst, reduce_op, E, y2, msg_op, scale_src, scale_dst, max_degree, out,
+                         packed, accumulate)
     if out is None:
         out = torch.empty((n_dst, D), dtype=torch.float32, device=dev)
     if isinstance(packed, NarrowPlan):
@@ -301,6 +337,33 @@ def _spmm_raw(indptr, cols, x2, n_dst, reduce_op, eid=None, y2=None, y_bcast=BCA
             _ptr(scale_dst), _ptr(packed[0]) if packed is not None else None, int(max_degree),
             (1 if accumulate else 0) | (2 if (packed is not None and packed[1]) else 0), _ptr(ws),
             wsn, _stream()))
+    return out
+
+
+def _spmm_x16(indptr, cols, x2, n_dst, reduce_op, E, y2, msg_op, scale_src, scale_dst, max_degree, out, packed,
+              accumulate):
+    """_spmm_raw for bfloat16 / float16 x: copy messages only, output in x's dtype (pglb_spmm_csr_x16)."""
+    if msg_op != "copy" or y2 is not None or accumulate:
+        raise TypeError("pgl_b200: 16-bit features aggregate copy messages only (got msg_op=%s%s%s)"
+                        % (msg_op, ", an edge operand" if y2 is not None else "", ", accumulate" if accumulate else ""))
+    dev = x2.device
+    D = int(x2.shape[1])
+    if out is None:
+        out = torch.empty((n_dst, D), dtype=x2.dtype, device=dev)
+    if isinstance(packed, NarrowPlan):
+        packed = packed.fallback() if packed.fallback is not None else None
+    need = ctypes.c_size_t(0)
+    check(lib.pglb_spmm_csr_ws(n_dst, E, D, ctypes.byref(need)))
+    ws = workspace(dev, need.value)
+    sslot = None
+    if scale_src is not None and reduce_op in ("sum", "mean") and getattr(packed, "slot_scale", None) is not None:
+        sslot = packed.slot_scale(scale_src)
+    with torch.cuda.device(dev):
+        check(lib.pglb_spmm_csr_x16(
+            _ptr(indptr), _ptr(cols), _ptr(x2), x2.stride(0), _ptr(out), out.stride(0), n_dst, int(x2.shape[0]), E, D,
+            _DTYPE16[x2.dtype], REDUCE[reduce_op], _ptr(scale_src), _ptr(sslot), _ptr(scale_dst),
+            _ptr(packed[0]) if packed is not None else None, int(max_degree),
+            2 if (packed is not None and packed[1]) else 0, _ptr(ws), ws.numel(), _stream()))
     return out
 
 
@@ -586,13 +649,17 @@ class _MaxMinAgg(torch.autograd.Function):
         if bwd is None:
             raise RuntimeError("pgl_b200: backward of this aggregation needs the reverse CSR")
         x2, out = ctx.saved_tensors
+        dtype = x2.dtype
+        if dtype in HALF_DTYPES:
+            # widening is exact, so the fp32 kernel's equality test x == out picks the same entries
+            x2, out, g = x2.float(), out.float(), g.float()
         g = g.contiguous()
         gx = torch.empty_like(x2)
         with torch.cuda.device(x2.device):
             check(lib.pglb_maxmin_bwd_f32(_ptr(bwd["indptr"]), _ptr(bwd["cols"]), _ptr(x2), _ptr(out),
                                           _ptr(g), _ptr(gx), int(x2.shape[0]), int(x2.shape[1]),
                                           _stream()))
-        return gx, None, None, None, None
+        return gx.to(dtype), None, None, None, None
 
 
 # rows of <= 64 floats: spmm_narrow2_kernel by default; PGLB_NARROW=1 PGLB_NARROW2=0 selects round 1's narrow kernel
@@ -637,9 +704,15 @@ def narrow_plan(indptr, cols, n_src, row_bytes=64):
 
 def _packed_of(csr, x2):
     """Per-(graph, row width) index data from the EdgeIndex cache: packed column ids (+ optional L2 hints) for the
-    wide-row kernels (64 < D <= 128), the narrow plan for D <= 64."""
+    wide-row kernels (64 < D <= 128), the narrow plan for D <= 64.  16-bit rows: packed ids for the rows the wide-row
+    kernel takes (64 < D <= 128, D % 8 == 0), with the hot set chosen for their real size; None otherwise."""
     fn = csr.get("packed")
     D = int(x2.shape[1])
+    if x2.dtype in HALF_DTYPES:
+        if fn is None or D > 128 or D <= 64 or D % 8:
+            return None
+        pk = fn(int(x2.shape[0]), D * x2.element_size())
+        return PackedCols(pk, csr.get("slot_scale")) if pk is not None else None
     if fn is None or D > 128 or D % 4 or (D <= 64 and not (NARROW_ROWS or NARROW2)):
         return None
     n_src = int(x2.shape[0])
@@ -654,12 +727,13 @@ def _packed_of(csr, x2):
     return PackedCols(pk, csr.get("slot_scale")) if pk is not None else None
 
 
-@f64_through
+@native16_through
 def aggregate_copy(x, fwd, n_dst, reduce_op="sum", bwd=None, scale_src=None, scale_dst=None):
-    """send_u_recv on a cached dst-CSR.  fwd/bwd: dicts {indptr, cols, degree, max_degree}."""
+    """send_u_recv on a cached dst-CSR.  fwd/bwd: dicts {indptr, cols, degree, max_degree}.  float32, bfloat16 or
+    float16 x; the output has x's dtype."""
     require_cuda(x)
     shape = x.shape
-    x2 = _f32_2d(x)
+    x2 = _f32_2d(x, allow16=True)
     needs_grad = x2.requires_grad and torch.is_grad_enabled()
     if reduce_op in ("sum", "mean") and needs_grad:
         out = _CopyAgg.apply(x2, fwd, bwd, n_dst, reduce_op, scale_src, scale_dst)
@@ -844,6 +918,11 @@ class _SegmentReduce(torch.autograd.Function):
     def backward(ctx, g):
         indptr, cols, pool_type, n_slots = ctx.meta
         d2, out = ctx.saved_tensors
+        dtype = d2.dtype
+        if dtype in HALF_DTYPES:
+            # the gradient is formed in fp32 (counts exact, sums over out-edges accumulated in fp32) and rounded once;
+            # widening is exact, so max / min select the same entries
+            d2, out, g = d2.float(), out.float(), g.float()
         g = g.contiguous()
         K = int(indptr.shape[0]) - 1
         counts = indptr[1:] - indptr[:-1]
@@ -855,18 +934,19 @@ class _SegmentReduce(torch.autograd.Function):
             src_rows = d2 if cols is None else gather_rows(d2, cols)
             ge = ge * (src_rows == gather_rows(out, seg)).to(ge.dtype)
         if cols is None:
-            return ge, None, None, None, None, None
+            return ge.to(dtype), None, None, None, None, None
         gd = torch.zeros_like(d2).index_add_(0, cols, ge)
-        return gd, None, None, None, None, None
+        return gd.to(dtype), None, None, None, None, None
 
 
-@f64_through
+@native16_through
 def segment_reduce(data, segment_ids, pool_type, num_segments=None, indptr=None, cols=None,
                    max_degree=-1):
     """paddle.geometric.segment_* over sorted ids (reference pgl/math.py:36-42).
-    `cols` (optional) fuses a row gather: slot j reads data[cols[j]] (lazy messages)."""
+    `cols` (optional) fuses a row gather: slot j reads data[cols[j]] (lazy messages).  float32, bfloat16 or float16
+    data; the output has data's dtype."""
     require_cuda(data)
-    d2 = _f32_2d(data)
+    d2 = _f32_2d(data, allow16=True)
     if indptr is None:
         ids = _i64(segment_ids)
         E = int(ids.shape[0])
