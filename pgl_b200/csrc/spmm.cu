@@ -502,18 +502,6 @@ int spmm_stream_run_x16(int dtype, const int64_t *indptr, const int64_t *cols, c
                         const float *scale_src, const float *scale_slot, const float *scale_dst, const uint32_t *cols32,
                         int l2_hints, void *ws, size_t ws_bytes, cudaStream_t stream);
 
-bool stream_narrow_enabled();  // PGLB_NARROW=1: experimental narrow-row streaming kernel (spmm_stream.cu)
-
-static bool use_stream_path() {
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("PGLB_SPMM_IMPL");
-        v = (e && strcmp(e, "legacy") == 0) ? 0 : 1;
-    }
-    return v == 1;
-}
-
-
 // The node-parallel launch sequence behind both entries: spmm_csr kernel over all rows, then, when some row is longer
 // than HUB_T slots, the hub plan and the two hub passes.  x / out are float, or 16-bit for pglb_spmm_csr_x16.
 // k_main runs over the rows, k_chunk turns hub chunks into fp32 partials, k_merge reduces a hub's partials into its row.
@@ -699,8 +687,7 @@ extern "C" int pglb_spmm_csr_slot_scale_f32(const int64_t *indptr, const int64_t
     const bool ue_fast = mode == 1 && D <= 128 && scale_src == nullptr && num_edges < 0x7fffffffLL &&
                          (msg_op == PGLB_MSG_MUL || msg_op == PGLB_MSG_ADD) &&
                          (y_bcast == PGLB_BCAST_SCALAR || (y_bcast == PGLB_BCAST_HEAD && head_dim % 4 == 0));
-    const bool narrow = mode == 0 && D <= 64 && reduce_op < PGLB_REDUCE_MAX && stream_narrow_enabled();
-    if ((mode == 0 || ue_fast) && vec4 && (D > 64 || narrow) && num_edges > 0 && use_stream_path()) {
+    if ((mode == 0 || ue_fast) && vec4 && D > 64 && num_edges > 0) {
         PGLB_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
                        "pglb_spmm_csr_f32: workspace must be 256-byte aligned");
         return spmm_stream_run(indptr, cols, x, ldx, out, ldo, n_dst, n_src, num_edges, D,
@@ -736,8 +723,7 @@ extern "C" int pglb_spmm_csr_x16(const int64_t *indptr, const int64_t *cols, con
     PGLB_CHECK_ARG(num_edges == 0 || x, PGLB_EINVAL, "pglb_spmm_csr_x16: x is NULL");
     PGLB_CHECK_ARG(ldx >= D && ldo >= D, PGLB_ESHAPE, "pglb_spmm_csr_x16: leading dimension smaller than D");
     PGLB_CHECK_ARG(D <= INT32_MAX, PGLB_ESHAPE, "pglb_spmm_csr_x16: D too large");
-    if (num_edges > 0 && use_stream_path() &&
-        stream_x16_eligible(cols, cols_packed, x, ldx, out, ldo, n_src, num_edges, D, reduce_op)) {
+    if (num_edges > 0 && stream_x16_eligible(cols, cols_packed, x, ldx, out, ldo, n_src, num_edges, D, reduce_op)) {
         PGLB_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
                        "pglb_spmm_csr_x16: workspace must be 256-byte aligned");
         return spmm_stream_run_x16(dtype, indptr, cols, x, ldx, out, ldo, n_dst, num_edges, D, reduce_op,

@@ -65,7 +65,6 @@ struct StreamP {
     float slope;             // YM 2: LeakyReLU negative slope
     float *partial_ml;       // YM 2: [2*ntasks, 64] running (max, sum) of cut rows, per lane
     int accumulate;          // SUM only: out = (out_prev + sum) * scale_dst
-    int hot_mode;            // 1: hot=evict_last cold=evict_first, 2: hot=last cold=normal, 3: hot=normal cold=first
     unsigned *counter;       // task queue head of the persistent (DYN) kernels, zeroed by task_plan_kernel
     long long *trace;        // debug, nullable: [ntasks, 4] = (start ns, end ns, SM id, warp slot) per task (pglb_debug_task_trace)
     float *lse;              // YM 2, nullable: [n_rows, H] log-sum-exp of every non-empty row's logits (saved for backward)
@@ -88,11 +87,6 @@ __device__ __forceinline__ uint64_t policy_evict_last() {
 __device__ __forceinline__ uint64_t policy_evict_first() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;\n" : "=l"(p));
-    return p;
-}
-__device__ __forceinline__ uint64_t policy_evict_normal() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;\n" : "=l"(p));
     return p;
 }
 __device__ __forceinline__ void cp_async4(unsigned smem_dst, const void *gsrc) {
@@ -218,23 +212,23 @@ __global__ void __launch_bounds__(256) task_plan_kernel(const int64_t *__restric
 // ---------------------------------------------------------------------------------------------
 // D <= 128 (one float4 per lane per row)
 // ---------------------------------------------------------------------------------------------
-// Ring geometry of the D <= 128 kernel.  CFG 0: 32 slots per lane, groups of 8, 7 warps per block
-// (14 per SM).  CFG 1: 16 slots, groups of 4, 14 warps per block (28 per SM): same bytes in flight
-// per SM, twice the warps to hide issue and shared-memory latency.
-template <int CFG, int YM>
+// Ring geometry of the D <= 128 kernel: 16 slots per lane, groups of 4, 14 warps per block (28 per SM).  That is the
+// bytes in flight per SM of a 32-slot ring with half the warps, and twice the warps to hide issue and shared-memory
+// latency.
+template <int YM>
 struct Geo {
-    static constexpr int kRing = CFG == 0 ? 32 : 16;
-    static constexpr int kGrp = CFG == 0 ? 8 : 4;
+    static constexpr int kRing = 16;
+    static constexpr int kGrp = 4;
     static constexpr int kLag = 3;
-    static constexpr int kWarps = CFG == 0 ? (YM ? 5 : 7) : (YM ? 11 : 14);
+    static constexpr int kWarps = YM ? 11 : 14;
     static constexpr int kGpb = 32 / kGrp;       // groups per 32-slot column batch
     static constexpr int kRg = kRing / kGrp;     // groups per turn of the ring
     static constexpr int kSmem = kWarps * kRing * (512 + (YM ? 128 : 0));
 };
 
-template <int RK, bool SCALED, int PK, int YM, int CFG>
-__global__ void __launch_bounds__(Geo<CFG, YM>::kWarps * 32, 2) spmm_stream128_kernel(const StreamP p) {
-    typedef Geo<CFG, YM> G_;
+template <int RK, bool SCALED, int PK, int YM>
+__global__ void __launch_bounds__(Geo<YM>::kWarps * 32, 2) spmm_stream128_kernel(const StreamP p) {
+    typedef Geo<YM> G_;
     constexpr int RING = G_::kRing, GRP = G_::kGrp, LAG = G_::kLag, GPB = G_::kGpb, RG = G_::kRg;
     // YM 1: message = x[src] (mul|add) y[eid, head(lane)] (send_ue_recv with a per-head or scalar
     // edge operand, the GAT aggregation): the 4-byte operand of every edge rides in a second
@@ -245,8 +239,8 @@ __global__ void __launch_bounds__(Geo<CFG, YM>::kWarps * 32, 2) spmm_stream128_k
     // kept with evict_last, the long tail streams through with evict_first so it cannot flush
     // them).
     constexpr bool HOT = (PK == 2);
-    const uint64_t pol_last = !HOT ? 0 : (p.hot_mode == 3 ? policy_evict_normal() : policy_evict_last());
-    const uint64_t pol_first = !HOT ? 0 : (p.hot_mode == 2 ? policy_evict_normal() : policy_evict_first());
+    const uint64_t pol_last = !HOT ? 0 : policy_evict_last();
+    const uint64_t pol_first = !HOT ? 0 : policy_evict_first();
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31;
     const int wib = threadIdx.x >> 5;
@@ -863,251 +857,6 @@ static int launch_empty_rows(const StreamP &p, cudaStream_t stream) {
     return PGLB_OK;
 }
 
-// ---------------------------------------------------------------------------------------------
-// Narrow rows (D <= 64 floats): EPW edges per warp step.  EXPERIMENTAL (PGLB_NARROW=1), written after
-// round 1's GPU budget was spent and NOT yet run on hardware.  Purpose: the column-sharded multi-GPU
-// layout (every GPU holds all rows but D/R columns and the whole CSR, no halo exchange at all), where
-// rows are 64 / 32 / 16 floats wide.  The wide kernel above spends the same ~45 warp instructions per
-// edge whatever the row width, so at D = 16 it would move 1/8 of the bytes in the same time.  Here a
-// warp step covers EPW = 2 / 4 / 8 consecutive slots: lane = sub * LPR + li, sub = which slot of the
-// step, li = which float4 of the row (LPR = 32 / EPW lanes per row).  Every lane still owns a private
-// 16-byte ring position per step, so the cp.async / wait / lds protocol is unchanged; what changes is
-// the row bookkeeping (a row may end inside a step) and the row epilogue (xor-shuffle reduce of the EPW
-// per-sub accumulators).  Sum / mean only; the per-row summation order is (sub-strided partial sums,
-// then tree) instead of sequential, so results agree with the oracle to rounding, not bit for bit.
-// Shares task planning, cut-row partials and the fix-up kernel with the wide kernel.
-template <int EPW, bool SCALED, int PK>
-__global__ void __launch_bounds__(Geo<1, 0>::kWarps * 32, 2) spmm_narrow_kernel(const StreamP p) {
-    typedef Geo<1, 0> G_;
-    constexpr int RING = G_::kRing, GRP = G_::kGrp, LAG = G_::kLag, RG = G_::kRg, W = G_::kWarps;
-    constexpr int LPR = 32 / EPW;                 // lanes per row
-    constexpr int SPG = GRP * EPW;                // slots per commit group
-    constexpr int GPB = 32 / SPG;                 // groups per 32-slot column batch (EPW 8 -> 1)
-    static_assert(SPG <= 32 && 32 % SPG == 0, "group must divide a column batch");
-    constexpr bool HOT = (PK == 2);
-    const uint64_t pol_last = !HOT ? 0 : (p.hot_mode == 3 ? policy_evict_normal() : policy_evict_last());
-    const uint64_t pol_first = !HOT ? 0 : (p.hot_mode == 2 ? policy_evict_normal() : policy_evict_first());
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    const int lane = threadIdx.x & 31;
-    const int wib = threadIdx.x >> 5;
-    const int sub = lane / LPR, li = lane % LPR;
-    const int64_t task = (int64_t)blockIdx.x * W + wib;
-    if (task >= p.ntasks) return;
-    const unsigned ring = (unsigned)__cvta_generic_to_shared(smem_raw) + wib * (RING * 512) + lane * 16;
-    const bool act = li * 4 < p.D;
-    const char *xlane = reinterpret_cast<const char *>(p.x) + (act ? li * 16 : 0);
-    const unsigned row_bytes = (unsigned)(p.ldx * 4);
-
-    const int64_t a = ld_ro(p.start + task);
-    const int64_t b = ld_ro(p.start + task + 1);
-    const int cnt = (int)(b - a);
-    int64_t row = ld_ro(p.first_row + task);
-    int64_t tail = -1;
-    if (cnt > 0) {
-        auto rel = [&](int64_t v) -> int {
-            const int64_t d = v - a;
-            return d < -(1 << 30) ? -(1 << 30) : (d > (1 << 30) ? (1 << 30) : (int)d);
-        };
-        int beg_rel = rel(ld_ro(p.indptr + row));
-        int end_rel = rel(ld_ro(p.indptr + row + 1));
-        int nxt_rel = (row + 2 <= p.n_rows) ? rel(ld_ro(p.indptr + row + 2)) : (1 << 30);
-        bool head = beg_rel < 0;
-        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-
-        auto reduce_subs = [&]() {  // every lane ends up with the sum over the EPW subs of its li
-#pragma unroll
-            for (int o = LPR; o < 32; o <<= 1) {
-                acc.x = __fadd_rn(acc.x, __shfl_xor_sync(0xffffffffu, acc.x, o));
-                acc.y = __fadd_rn(acc.y, __shfl_xor_sync(0xffffffffu, acc.y, o));
-                acc.z = __fadd_rn(acc.z, __shfl_xor_sync(0xffffffffu, acc.z, o));
-                acc.w = __fadd_rn(acc.w, __shfl_xor_sync(0xffffffffu, acc.w, o));
-            }
-        };
-        const bool writer = act && sub == 0;
-
-        auto finish_row = [&]() {
-            reduce_subs();
-            if (head) {
-                if (writer) *reinterpret_cast<float4 *>(p.partial + (2 * task) * p.dpad + li * 4) = acc;
-                head = false;
-            } else if (writer) {
-                float4 v = acc;
-                const int deg = end_rel - beg_rel;
-                if (deg == 0) v = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (p.accumulate) {
-                    const float4 o = *reinterpret_cast<const float4 *>(p.out + row * p.ldo + li * 4);
-                    v.x = __fadd_rn(o.x, v.x); v.y = __fadd_rn(o.y, v.y);
-                    v.z = __fadd_rn(o.z, v.z); v.w = __fadd_rn(o.w, v.w);
-                }
-                if (p.reduce_op == PGLB_REDUCE_MEAN && deg != 0) {
-                    const float c = (float)deg;
-                    v.x = __fdiv_rn(v.x, c); v.y = __fdiv_rn(v.y, c);
-                    v.z = __fdiv_rn(v.z, c); v.w = __fdiv_rn(v.w, c);
-                }
-                if (p.scale_dst) {
-                    const float sd = __ldg(p.scale_dst + row);
-                    v.x = __fmul_rn(v.x, sd); v.y = __fmul_rn(v.y, sd);
-                    v.z = __fmul_rn(v.z, sd); v.w = __fmul_rn(v.w, sd);
-                }
-                __stcs(reinterpret_cast<float4 *>(p.out + row * p.ldo + li * 4), v);
-            }
-            ++row;
-            beg_rel = end_rel;
-            end_rel = nxt_rel;
-            nxt_rel = (row + 2 <= p.n_rows) ? rel(ld_ro(p.indptr + row + 2)) : (1 << 30);
-            if (end_rel == beg_rel && row < p.n_rows) {  // run of empty rows: jump (see the wide kernel)
-                const int64_t pos_abs = a + beg_rel;
-                if (pos_abs >= p.E) {
-                    row = p.n_rows;
-                    end_rel = 1 << 30;
-                } else {
-                    row = row_of_slot_from(p.indptr, p.n_rows, row, pos_abs);
-                    end_rel = rel(ld_ro(p.indptr + row + 1));
-                    nxt_rel = (row + 2 <= p.n_rows) ? rel(ld_ro(p.indptr + row + 2)) : (1 << 30);
-                }
-            }
-            acc = make_float4(0.f, 0.f, 0.f, 0.f);
-        };
-
-        auto load_col = [&](int batch) -> unsigned {
-            const int j = batch * 32 + lane;
-            if (j >= cnt) return 0u;
-            if (PK != 0) return __ldcs(p.cols32 + a + j);
-            return (unsigned)(p.cols ? ld_stream(p.cols + a + j) : (a + j));
-        };
-        unsigned col_cur = load_col(0);
-        unsigned col_nxt = load_col(1);
-        // source scales of the column batches between the consume point and the issue point: the
-        // consumed group trails the issued one by LAG groups = up to ceil(LAG / GPB) batches
-        constexpr int SH = (LAG + GPB - 1) / GPB + 1;
-        float sc_hist[SH];
-#pragma unroll
-        for (int i = 0; i < SH; ++i) sc_hist[i] = 1.0f;
-        if (SCALED) sc_hist[0] = (lane < cnt) ? __ldg(p.scale_src + (col_cur & 0x7fffffffu)) : 1.0f;
-
-        const int ngroups = (cnt + SPG - 1) / SPG;
-#pragma unroll 1
-        for (int g = 0; g < ngroups + LAG; ++g) {
-            if (g < ngroups) {
-                const int gsub = g % GPB;  // position of the group inside its 32-slot column batch
-                if (gsub == 0 && g > 0) {
-                    col_cur = col_nxt;
-                    col_nxt = load_col(g / GPB + 1);
-                    if (SCALED) {
-#pragma unroll
-                        for (int i = SH - 1; i > 0; --i) sc_hist[i] = sc_hist[i - 1];
-                        sc_hist[0] = (g * SPG + lane < cnt) ? __ldg(p.scale_src + (col_cur & 0x7fffffffu)) : 1.0f;
-                    }
-                }
-                const int rs = g % RG;
-                const unsigned gaddr = ring + rs * (GRP * 512);
-#pragma unroll
-                for (int k = 0; k < GRP; ++k) {
-                    const int src_lane = (gsub * GRP + k) * EPW + sub;      // my slot inside the batch
-                    const unsigned c = __shfl_sync(0xffffffffu, col_cur, src_lane);
-                    const int my = (g * GRP + k) * EPW + sub;               // my slot inside the task
-                    if (my < cnt) {
-                        if (HOT) {
-                            const uint64_t pol = (c >> 31) ? pol_last : pol_first;
-                            cp_async16_hint(gaddr + k * 512, xlane + (size_t)(c & 0x7fffffffu) * row_bytes, pol);
-                        } else {
-                            cp_async16(gaddr + k * 512, xlane + (size_t)(c & 0x7fffffffu) * row_bytes);
-                        }
-                    }
-                }
-            }
-            cp_async_commit();
-            if (g >= LAG) {
-                cp_async_wait<LAG>();
-                const int gc = g - LAG;
-                const int csub = gc % GPB;
-                const int crs = gc % RG;
-                const int bcur = (g < ngroups ? g : ngroups - 1) / GPB;  // batch held by sc_hist[0]
-                const int back = bcur - gc / GPB;                        // 0 .. SH - 1
-                float sc_reg = sc_hist[0];
-#pragma unroll
-                for (int i = 1; i < SH; ++i)
-                    if (back == i) sc_reg = sc_hist[i];
-                const unsigned gaddr = ring + crs * (GRP * 512);
-#pragma unroll 1
-                for (int k = 0; k < GRP; ++k) {
-                    const int s0 = (gc * GRP + k) * EPW;   // first slot of this step
-                    if (s0 >= cnt) break;
-                    const int hi = (s0 + EPW < cnt) ? s0 + EPW : cnt;
-                    const int my = s0 + sub;
-                    const float4 v = lds128(gaddr + k * 512);
-                    float s = 1.0f;
-                    if (SCALED) s = __shfl_sync(0xffffffffu, sc_reg, (csub * GRP + k) * EPW + sub);
-                    while (end_rel <= s0) finish_row();   // rows (and empty rows) that ended before this step
-                    int lo = s0;
-                    while (true) {
-                        const int e = end_rel < hi ? end_rel : hi;
-                        if (my >= lo && my < e) {
-                            if (SCALED) {
-                                acc.x = fmaf(v.x, s, acc.x); acc.y = fmaf(v.y, s, acc.y);
-                                acc.z = fmaf(v.z, s, acc.z); acc.w = fmaf(v.w, s, acc.w);
-                            } else {
-                                acc.x = __fadd_rn(acc.x, v.x); acc.y = __fadd_rn(acc.y, v.y);
-                                acc.z = __fadd_rn(acc.z, v.z); acc.w = __fadd_rn(acc.w, v.w);
-                            }
-                        }
-                        if (end_rel < hi) {   // the row ends inside this step: the next one starts at end_rel
-                            lo = end_rel;
-                            finish_row();
-                        } else {
-                            break;
-                        }
-                    }
-                }
-            }
-        }
-        while (row < p.n_rows && end_rel <= cnt) finish_row();
-        if (row < p.n_rows && beg_rel < cnt) {
-            reduce_subs();
-            if (writer)
-                *reinterpret_cast<float4 *>(p.partial + (head ? (2 * task) : (2 * task + 1)) * p.dpad + li * 4) = acc;
-            if (!head) tail = row;
-        }
-    }
-    if (lane == 0) p.tail_row[task] = tail;
-}
-
-static int narrow_mode() {
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("PGLB_NARROW");
-        v = (e && atoi(e) == 1) ? 1 : 0;  // round 1's narrow kernel: validated in round 2, superseded by spmm_narrow2 (opt-in)
-    }
-    return v;
-}
-
-bool stream_narrow_enabled() { return narrow_mode() == 1; }
-
-template <int EPW, bool SCALED, int PK>
-static int launch_narrow(const StreamP &p, cudaStream_t stream) {
-    typedef Geo<1, 0> G_;
-    constexpr int W = G_::kWarps;
-    static std::atomic<unsigned long long> attr_done{0};
-    PGLB_CUDA(ensure_dyn_smem(spmm_narrow_kernel<EPW, SCALED, PK>, G_::kSmem, attr_done));
-    const int64_t blocks = (p.ntasks + W - 1) / W;
-    PGLB_CHECK_ARG(blocks <= 0x7fffffffLL, PGLB_ESHAPE, "spmm_narrow: grid too large");
-    spmm_narrow_kernel<EPW, SCALED, PK><<<(unsigned)blocks, W * 32, G_::kSmem, stream>>>(p);
-    PGLB_LAUNCH_CHECK("spmm_narrow_kernel");
-    const int64_t fblocks = (p.ntasks * 32 + 255) / 256;
-    spmm_stream_fixup_kernel<1, 0><<<(unsigned)fblocks, 256, 0, stream>>>(p);
-    PGLB_LAUNCH_CHECK("spmm_stream_fixup_kernel");
-    return PGLB_OK;
-}
-
-template <int EPW>
-static int launch_narrow_pk(const StreamP &p, int pk, bool scaled, cudaStream_t stream) {
-    if (scaled)
-        return pk == 2 ? launch_narrow<EPW, true, 2>(p, stream)
-                       : pk == 1 ? launch_narrow<EPW, true, 1>(p, stream) : launch_narrow<EPW, true, 0>(p, stream);
-    return pk == 2 ? launch_narrow<EPW, false, 2>(p, stream)
-                   : pk == 1 ? launch_narrow<EPW, false, 1>(p, stream) : launch_narrow<EPW, false, 0>(p, stream);
-}
-
 #include "spmm_v5.inl"
 #include "spmm_gat5.inl"
 #include "spmm_narrow2.inl"
@@ -1211,26 +960,17 @@ static long long *trace_for(int64_t ntasks) {
     return (t && ntasks <= g_trace_cap.load(std::memory_order_acquire)) ? t : nullptr;
 }
 
-static int stream_cfg() {
-    static int c = -1;
-    if (c < 0) {
-        const char *e = getenv("PGLB_STREAM_CFG");
-        c = (e && atoi(e) == 0) ? 0 : 1;
-    }
-    return c;
-}
-
-template <int RK, bool SCALED, int PK, int YM, int CFG>
-static int launch_stream128_cfg(const StreamP &p, cudaStream_t stream) {
-    typedef Geo<CFG, YM> G_;
+template <int RK, bool SCALED, int PK, int YM>
+static int launch_stream128(const StreamP &p, cudaStream_t stream) {
+    typedef Geo<YM> G_;
     constexpr int W = G_::kWarps;
     const int smem = G_::kSmem;
     static std::atomic<unsigned long long> attr_done{0};
-    PGLB_CUDA(ensure_dyn_smem(spmm_stream128_kernel<RK, SCALED, PK, YM, CFG>, smem, attr_done));
+    PGLB_CUDA(ensure_dyn_smem(spmm_stream128_kernel<RK, SCALED, PK, YM>, smem, attr_done));
     int64_t blocks = (p.ntasks + W - 1) / W;
     PGLB_CHECK_ARG(blocks <= 0x7fffffffLL, PGLB_ESHAPE, "spmm_stream: grid too large");
     if (p.dyn && blocks > (int64_t)sm_count() * 2) blocks = (int64_t)sm_count() * 2;   // persistent: 2 CTAs per SM
-    spmm_stream128_kernel<RK, SCALED, PK, YM, CFG><<<(unsigned)blocks, W * 32, smem, stream>>>(p);
+    spmm_stream128_kernel<RK, SCALED, PK, YM><<<(unsigned)blocks, W * 32, smem, stream>>>(p);
     PGLB_LAUNCH_CHECK("spmm_stream128_kernel");
     const int64_t fblocks = (p.ntasks * 32 + 255) / 256;
     if (YM == 2) {
@@ -1240,12 +980,6 @@ static int launch_stream128_cfg(const StreamP &p, cudaStream_t stream) {
     }
     PGLB_LAUNCH_CHECK("spmm_stream_fixup_kernel");
     return PGLB_OK;
-}
-
-template <int RK, bool SCALED, int PK, int YM>
-static int launch_stream128(const StreamP &p, cudaStream_t stream) {
-    return stream_cfg() == 0 ? launch_stream128_cfg<RK, SCALED, PK, YM, 0>(p, stream)
-                             : launch_stream128_cfg<RK, SCALED, PK, YM, 1>(p, stream);
 }
 
 template <int ITERS, int RK>
@@ -1297,15 +1031,6 @@ static int stream_prepare(StreamP &p, const int64_t *indptr, const int64_t *cols
     p.dpad = w.dpad;
     p.tail_row = w.tail_row;
     p.cols32 = cols32;
-    {
-        static int mode = 0;
-        if (mode == 0) {
-            const char *e = getenv("PGLB_HOT_MODE");
-            mode = e ? atoi(e) : 1;
-            if (mode < 1 || mode > 3) mode = 1;
-        }
-        p.hot_mode = mode;
-    }
     p.counter = w.counter;
     p.dyn = dyn_mode("PGLB_V5_DYN", 0, w.ntasks);
     p.trace = trace_for(w.ntasks);
@@ -1345,13 +1070,6 @@ int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, 
     const int64_t cv = D / 4;
     const int rk = (reduce_op >= PGLB_REDUCE_MAX) ? 1 : 0;
     const bool small_ids = (cols ? n_src : E) < 0x7fffffffLL && ldx * 4 < 0xffffffffLL;
-    if (narrow_mode() && !y && rk == 0 && cv <= 16 && small_ids) {
-        // EXPERIMENTAL narrow-row path (PGLB_NARROW=1): 2 / 4 / 8 slots per warp step
-        const int pk = (cols32 && cols) ? (l2_hints ? 2 : 1) : 0;
-        if (cv <= 4) return launch_narrow_pk<8>(p, pk, scale_src != nullptr, stream);
-        if (cv <= 8) return launch_narrow_pk<4>(p, pk, scale_src != nullptr, stream);
-        return launch_narrow_pk<2>(p, pk, scale_src != nullptr, stream);
-    }
     if (cv <= 32 && v5_eligible(p, n_src, rk, small_ids))
         return launch_v5(p, cols32 != nullptr && cols != nullptr && l2_hints != 0, stream);
     p.dyn = dyn_mode("PGLB_S128_DYN", 2, p.ntasks);   // round 1's kernel (max / min, edge operands): descending queue
@@ -1378,7 +1096,7 @@ int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, 
 // kernel (spmm.cu).
 bool stream_x16_eligible(const int64_t *cols, const uint32_t *cols32, const void *x, int64_t ldx, const void *out,
                          int64_t ldo, int64_t n_src, int64_t E, int64_t D, int reduce_op) {
-    if (v5_mode() == 0 || reduce_op >= PGLB_REDUCE_MAX || D <= 64 || D > 128 || D % 8 != 0) return false;
+    if (reduce_op >= PGLB_REDUCE_MAX || D <= 64 || D > 128 || D % 8 != 0) return false;
     if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(out) & 15) || ldx % 8 || ldo % 8)
         return false;
     if ((cols ? n_src : E) >= 0x7fffffffLL || ldx * 2 >= 0xffffffffLL) return false;  // small_ids of the fp32 run
@@ -1422,38 +1140,24 @@ static int64_t narrow2_task_size(int64_t E, int64_t D) {
 }
 size_t narrow2_ws_bytes(int64_t E, int64_t D) { return stream_layout(nullptr, E, D, narrow2_task_size(E, D)).bytes; }
 
-static int narrow2_u() {
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("PGLB_NARROW_U");
-        v = (e && atoi(e) == 4) ? 4 : 8;
-    }
-    return v;
-}
-
 template <int L>
-static void launch_narrow2(const NarrowP &p, int sc, bool hot, int u, unsigned blocks, cudaStream_t stream) {
-#define PGLB_N2K(SC, MN, HT, UU) spmm_narrow2_kernel<L, SC, MN, HT, UU><<<blocks, kNarrowWarps * 32, 0, stream>>>(p)
-    if (p.mean) {  // mean (GraphSAGE): no L2 hints, 8 in flight
-        if (sc == 1) PGLB_N2K(1, true, false, 8);
-        else if (sc == 2) PGLB_N2K(2, true, false, 8);
-        else PGLB_N2K(0, true, false, 8);
+static void launch_narrow2(const NarrowP &p, int sc, bool hot, unsigned blocks, cudaStream_t stream) {
+#define PGLB_N2K(SC, MN, HT) spmm_narrow2_kernel<L, SC, MN, HT><<<blocks, kNarrowWarps * 32, 0, stream>>>(p)
+    if (p.mean) {  // mean (GraphSAGE): no L2 hints
+        if (sc == 1) PGLB_N2K(1, true, false);
+        else if (sc == 2) PGLB_N2K(2, true, false);
+        else PGLB_N2K(0, true, false);
         return;
     }
-#define PGLB_N2S(SC)                                     \
-    do {                                                 \
-        if (hot) {                                       \
-            if (u == 4) PGLB_N2K(SC, false, true, 4);    \
-            else PGLB_N2K(SC, false, true, 8);           \
-        } else {                                         \
-            if (u == 4) PGLB_N2K(SC, false, false, 4);   \
-            else PGLB_N2K(SC, false, false, 8);          \
-        }                                                \
-    } while (0)
-    if (sc == 1) PGLB_N2S(1);
-    else if (sc == 2) PGLB_N2S(2);
-    else PGLB_N2S(0);
-#undef PGLB_N2S
+    if (hot) {
+        if (sc == 1) PGLB_N2K(1, false, true);
+        else if (sc == 2) PGLB_N2K(2, false, true);
+        else PGLB_N2K(0, false, true);
+    } else {
+        if (sc == 1) PGLB_N2K(1, false, false);
+        else if (sc == 2) PGLB_N2K(2, false, false);
+        else PGLB_N2K(0, false, false);
+    }
 #undef PGLB_N2K
 }
 
@@ -1480,15 +1184,6 @@ int narrow2_run(const uint32_t *plan, const int32_t *nz_row, const int32_t *blk_
     p.scale_src = scale_src;
     p.sval = sval;
     p.scale_dst = scale_dst;
-    {
-        static int mode = 0;
-        if (mode == 0) {
-            const char *e = getenv("PGLB_HOT_MODE");
-            mode = e ? atoi(e) : 1;
-            if (mode < 1 || mode > 3) mode = 1;
-        }
-        p.hot_mode = mode;
-    }
     p.T = T;
     p.ntasks = w.ntasks;
     p.partial = w.partial;
@@ -1517,9 +1212,9 @@ int narrow2_run(const uint32_t *plan, const int32_t *nz_row, const int32_t *blk_
     PGLB_CHECK_ARG(blocks <= 0x7fffffffLL, PGLB_ESHAPE, "spmm_narrow2: grid too large");
     const int lpr = narrow2_lpr(D);
     const int sc = sval ? 2 : (scale_src ? 1 : 0);
-    if (lpr == 4) launch_narrow2<4>(p, sc, hot != 0, narrow2_u(), (unsigned)blocks, stream);
-    else if (lpr == 8) launch_narrow2<8>(p, sc, hot != 0, narrow2_u(), (unsigned)blocks, stream);
-    else launch_narrow2<16>(p, sc, hot != 0, narrow2_u(), (unsigned)blocks, stream);
+    if (lpr == 4) launch_narrow2<4>(p, sc, hot != 0, (unsigned)blocks, stream);
+    else if (lpr == 8) launch_narrow2<8>(p, sc, hot != 0, (unsigned)blocks, stream);
+    else launch_narrow2<16>(p, sc, hot != 0, (unsigned)blocks, stream);
     PGLB_LAUNCH_CHECK("spmm_narrow2_kernel");
     const int64_t fblocks = (p.ntasks * 32 + 255) / 256;
     spmm_stream_fixup_kernel<1, 0><<<(unsigned)fblocks, 256, 0, stream>>>(sp);
@@ -1562,7 +1257,6 @@ int gat_fused_run(const int64_t *indptr, const int64_t *cols, const float *f, in
     p.head_dim = (int)(D / H);
     p.attn_dst = attn_dst;
     p.slope = slope;
-    p.hot_mode = 1;
     p.counter = w.counter;
     p.dyn = dyn_mode("PGLB_GAT_DYN", 1, w.ntasks);
     p.trace = trace_for(w.ntasks);

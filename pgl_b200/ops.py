@@ -319,7 +319,7 @@ def _spmm_raw(indptr, cols, x2, n_dst, reduce_op, eid=None, y2=None, y_bcast=BCA
                                                _ptr(sval), _ptr(scale_dst), 2 if packed.hints else 0, _ptr(ws),
                                                ws.numel(), _stream()))
             return out
-        packed = packed.fallback() if packed.fallback is not None else None
+        packed = None
     need = ctypes.c_size_t(0)
     check(lib.pglb_spmm_csr_ws(n_dst, E, D, ctypes.byref(need)))
     ws = workspace(dev, need.value)
@@ -351,7 +351,7 @@ def _spmm_x16(indptr, cols, x2, n_dst, reduce_op, E, y2, msg_op, scale_src, scal
     if out is None:
         out = torch.empty((n_dst, D), dtype=x2.dtype, device=dev)
     if isinstance(packed, NarrowPlan):
-        packed = packed.fallback() if packed.fallback is not None else None
+        packed = None
     need = ctypes.c_size_t(0)
     check(lib.pglb_spmm_csr_ws(n_dst, E, D, ctypes.byref(need)))
     ws = workspace(dev, need.value)
@@ -662,11 +662,7 @@ class _MaxMinAgg(torch.autograd.Function):
         return gx.to(dtype), None, None, None, None
 
 
-# rows of <= 64 floats: spmm_narrow2_kernel by default; PGLB_NARROW=1 PGLB_NARROW2=0 selects round 1's narrow kernel
-NARROW2 = os.environ.get("PGLB_NARROW2", "1") != "0"          # spmm_narrow2_kernel for copy-sum / mean over rows of <= 64 floats
-NARROW_ROWS = os.environ.get("PGLB_NARROW") == "1"            # round 1's spmm_narrow_kernel (opt-in, superseded)
-
-
+# rows of <= 64 floats: spmm_narrow2_kernel for copy-sum / mean
 NARROW_HOT_BYTES = int(float(os.environ.get("PGLB_NARROW_HOT_MB", "64")) * (1 << 20))   # L2 residency budget, narrow rows
 NARROW_SLOT_SCALE = os.environ.get("PGLB_NARROW_SLOT_SCALE", "1") != "0"                 # stream cached per-slot norms
 
@@ -674,12 +670,12 @@ NARROW_SLOT_SCALE = os.environ.get("PGLB_NARROW_SLOT_SCALE", "1") != "0"        
 class NarrowPlan(object):
     """What pglb_spmm_narrow_f32 streams instead of cols / indptr (see include/pglb.h).  `hints`: bit 31 of the plan
     carries an L2 residency hint.  `slot_scale(scale_src)`: the source scale laid out per CSR slot (cached per scale
-    tensor by the EdgeIndex).  `fallback()` gives the packed column ids for calls the narrow kernel does not take."""
-    __slots__ = ("plan", "nz_row", "blk_k", "hints", "slot_scale", "fallback")
+    tensor by the EdgeIndex).  Calls the narrow kernel does not take run without packed ids."""
+    __slots__ = ("plan", "nz_row", "blk_k", "hints", "slot_scale")
 
-    def __init__(self, plan, nz_row, blk_k, hints=False, slot_scale=None, fallback=None):
+    def __init__(self, plan, nz_row, blk_k, hints=False, slot_scale=None):
         self.plan, self.nz_row, self.blk_k, self.hints = plan, nz_row, blk_k, bool(hints)
-        self.slot_scale, self.fallback = slot_scale, fallback
+        self.slot_scale = slot_scale
 
 
 def narrow_plan(indptr, cols, n_src, row_bytes=64):
@@ -713,15 +709,14 @@ def _packed_of(csr, x2):
             return None
         pk = fn(int(x2.shape[0]), D * x2.element_size())
         return PackedCols(pk, csr.get("slot_scale")) if pk is not None else None
-    if fn is None or D > 128 or D % 4 or (D <= 64 and not (NARROW_ROWS or NARROW2)):
+    if fn is None or D > 128 or D % 4:
         return None
     n_src = int(x2.shape[0])
-    if D <= 64 and NARROW2 and csr.get("plan") is not None and 0 < n_src < (1 << 30) and \
-            csr["cols"] is not None and int(csr["cols"].shape[0]) > 0:
-        plan, nz_row, blk_k, hints = csr["plan"](n_src, D * 4)
-        return NarrowPlan(plan, nz_row, blk_k, hints, slot_scale=csr.get("slot_scale"),
-                          fallback=(lambda: fn(n_src, D * 4)) if NARROW_ROWS else None)
-    if D <= 64 and not NARROW_ROWS:
+    if D <= 64:
+        if csr.get("plan") is not None and 0 < n_src < (1 << 30) and \
+                csr["cols"] is not None and int(csr["cols"].shape[0]) > 0:
+            plan, nz_row, blk_k, hints = csr["plan"](n_src, D * 4)
+            return NarrowPlan(plan, nz_row, blk_k, hints, slot_scale=csr.get("slot_scale"))
         return None
     pk = fn(n_src, D * 4)
     return PackedCols(pk, csr.get("slot_scale")) if pk is not None else None
@@ -1432,11 +1427,9 @@ def stream_kernel_name(num_edges=None, num_rows=None):
     take the groups-of-8 geometry)."""
     v = os.environ.get("PGLB_STREAM_V5", "1")
     g = os.environ.get("PGLB_V5_GEO")
-    if g not in ("0", "1", "2"):
+    if g not in ("0", "2"):
         g = "2" if (num_edges is not None and num_rows and num_edges >= 12 * num_rows) else "0"
-    geo = {"0": "GRP=4,NG=4,W=13", "1": "GRP=8,NG=4,W=6", "2": "GRP=8,NG=3,W=9"}[g]
-    if v == "0":
-        return "spmm_stream128_kernel<RK=0,SCALED=1,PK=2,YM=0,CFG=1> (+ task_plan, empty_rows, fix-up kernels)"
+    geo = {"0": "GRP=4,NG=4,W=13", "2": "GRP=8,NG=3,W=9"}[g]
     how = "bulk copy per row (cp.async.bulk)" if v != "2" else "LDGSTS ring"
     q = "" if os.environ.get("PGLB_V5_DYN") == "0" or v == "2" else ", device-side task queue"
     return "spmm_v5_kernel<%s, %s%s> (+ task_plan, empty_rows, fix-up kernels)" % (how, geo, q)

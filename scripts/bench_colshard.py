@@ -1,6 +1,6 @@
 """Column-sharded cfg5 aggregation (SURVEY 8e "alternative to measure") -- EXPERIMENTAL, never run.
 
-    PGLB_NARROW=1 python -m torch.distributed.run --nnodes=1 --nproc-per-node R --master-addr 127.0.0.1 \
+    python -m torch.distributed.run --nnodes=1 --nproc-per-node R --master-addr 127.0.0.1 \
         --master-port 29511 scripts/bench_colshard.py [--steps 10]
 
 Every rank builds the whole graph and owns 128/R feature columns.  Reports, max over ranks: the
@@ -67,7 +67,6 @@ def main():
         d = cs.d_local
         b_alg = args.edges * (4 * d + 8) + args.nodes * 4 * d + (args.nodes + 1) * 8 + 2 * args.nodes * 4
         print(json.dumps({"workload": "cfg5, column-sharded %d ways (%d columns per GPU)" % (world, d),
-                          "narrow_kernel": os.environ.get("PGLB_NARROW") == "1",
                           "aggregate_ms": t_agg, "reshard_all_to_all_ms": t_a2a, "aggregate_plus_reshard_ms": t_both,
                           "edges_per_s_aggregate": args.edges / (t_agg * 1e-3),
                           "edges_per_s_with_reshard": args.edges / (t_both * 1e-3),

@@ -1,5 +1,6 @@
 """Where does the groups-of-8 geometry of spmm_v5_kernel start to win?  Chung-Lu graphs (exponent 0.8, permuted ids) of
-2M nodes and 16 / 24 / 32 / 40 slots per row, 128-float rows, sum; run once per PGLB_V5_GEO (read once per process)."""
+2M nodes and 16 / 24 / 32 / 40 slots per row, 128-float rows, sum; run once with PGLB_V5_GEO=0 (groups of 4) and once
+with PGLB_V5_GEO=2 (groups of 8); the library reads it once per process."""
 import json
 import os
 import sys

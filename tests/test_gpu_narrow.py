@@ -1,8 +1,7 @@
-"""GPU tests of the narrow-row kernels: rows of <= 64 floats, the shapes of a column-sharded feature matrix.
-Default path: spmm_narrow2_kernel (csrc/spmm_narrow2.inl: sub-warp-major 32-slot ranges, plan with row-start flags).
-Round 1's spmm_narrow_kernel (csrc/spmm_stream.cu, PGLB_NARROW=1 PGLB_NARROW2=0) is kept as an opt-in and runs the same
-tests in a child process, as does the cut-row variant (PGLB_STREAM_TASK=64: tasks of one chunk, every long row cut) --
-these switches are read once per process by the library.
+"""GPU tests of the narrow-row kernel: rows of <= 64 floats, the shapes of a column-sharded feature matrix.
+spmm_narrow2_kernel (csrc/spmm_narrow2.inl: sub-warp-major 32-slot ranges, plan with row-start flags).  The cut-row
+variant (PGLB_STREAM_TASK=64: tasks of one chunk, every long row cut) runs the same tests in a child process -- the
+library reads that switch once per process.
 
 Sum order differs from the sequential oracle (ranges of a row are summed separately, then added), so the bar is the
 fp32 tolerance, not bit equality."""
@@ -104,8 +103,3 @@ def test_cut_rows_in_child_process():
     """The same tests with 64-slot tasks (rounded up to one chunk: every long row is cut; partials + fix-up work)."""
     _child({"PGLB_STREAM_TASK": "64"})
 
-
-def test_round1_narrow_kernel_in_child_process():
-    """Round 1's narrow kernel stays correct behind its switch (whole rows and cut rows)."""
-    _child({"PGLB_NARROW": "1", "PGLB_NARROW2": "0"})
-    _child({"PGLB_NARROW": "1", "PGLB_NARROW2": "0", "PGLB_STREAM_TASK": "64"})

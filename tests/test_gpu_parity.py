@@ -35,9 +35,8 @@ def check(out, want, max_row, narrow=False):
 
 
 def narrow_rows(D):
-    """widths the narrow-row kernel takes (csrc/spmm_narrow2.inl), unless it is switched off"""
-    import os
-    return D % 4 == 0 and D <= 64 and os.environ.get("PGLB_NARROW2", "1") != "0"
+    """widths the narrow-row kernel takes (csrc/spmm_narrow2.inl)"""
+    return D % 4 == 0 and D <= 64
 
 
 def rel_err(a, b):
