@@ -20,6 +20,7 @@
 #include <cfloat>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -277,24 +278,17 @@ __device__ __forceinline__ void spmm_csr_body(const SpmmP &p) {
     }
 }
 
-template <int VEC, int G, int ITERS, int MODE, int RK>
+template <typename TI, typename TO, int VEC, int G, int ITERS, int MODE, int RK>
 __global__ void __launch_bounds__(kThreads) spmm_csr_kernel(const SpmmP p) {
-    spmm_csr_body<float, float, VEC, G, ITERS, MODE, RK>(p);
-}
-// copy messages over 16-bit features (pglb_spmm_csr_x16): TI / TO as above
-template <typename TI, typename TO, int VEC, int G, int ITERS, int RK>
-__global__ void __launch_bounds__(kThreads) spmm_csr_x16_kernel(const SpmmP p) {
-    spmm_csr_body<TI, TO, VEC, G, ITERS, 0, RK>(p);
+    spmm_csr_body<TI, TO, VEC, G, ITERS, MODE, RK>(p);
 }
 // 4 elements per lane with 2 column iterations (129 <= D <= 256): under __launch_bounds__(kThreads)
 // ptxas holds these at 80 registers and spills 16-32 bytes; a cap of 96 registers instead removes the spills and ran
 // 11 % faster on an H100.  One element per lane (odd D, unaligned rows) also spills 8-24 bytes under the launch bound,
 // but capped it ran 17-26 % slower (more registers, fewer resident blocks), so it keeps the launch bound and its
 // spills, like the fp32 kernel of the same shape.
-template <int VEC, int ITERS>
-constexpr bool x16_capped() { return VEC == 4 && ITERS == 2; }
 template <typename TI, typename TO, int VEC, int G, int ITERS, int RK>
-__global__ void __maxnreg__(96) spmm_csr_x16_capped_kernel(const SpmmP p) {
+__global__ void __maxnreg__(96) spmm_csr_capped_kernel(const SpmmP p) {
     spmm_csr_body<TI, TO, VEC, G, ITERS, 0, RK>(p);
 }
 
@@ -391,54 +385,39 @@ static Shape pick_shape(int64_t D, bool vec4) {
 
 typedef void (*SpmmKernel)(const SpmmP);
 
-template <int VEC, int G, int ITERS>
+// TI / TO: element types of the kernel's x / out.  A 16-bit type on either side takes the capped kernel at 4 elements
+// per lane and two column iterations; MODE 1 (an edge operand) exists for float32 only.
+template <typename TI, typename TO, int VEC, int G, int ITERS>
 static SpmmKernel pick_mode(int mode, int rk) {
-    if (mode == 0) return rk == 0 ? spmm_csr_kernel<VEC, G, ITERS, 0, 0> : spmm_csr_kernel<VEC, G, ITERS, 0, 1>;
-    return rk == 0 ? spmm_csr_kernel<VEC, G, ITERS, 1, 0> : spmm_csr_kernel<VEC, G, ITERS, 1, 1>;
-}
-
-template <int VEC>
-static SpmmKernel pick_kernel_v(const Shape &s, int mode, int rk) {
-    switch (s.g) {
-        case 4: return pick_mode<VEC, 4, 1>(mode, rk);
-        case 8: return pick_mode<VEC, 8, 1>(mode, rk);
-        case 16: return pick_mode<VEC, 16, 1>(mode, rk);
-        default:
-            if (s.iters == 1) return pick_mode<VEC, 32, 1>(mode, rk);
-            if (s.iters == 2) return pick_mode<VEC, 32, 2>(mode, rk);
-            return pick_mode<VEC, 32, 4>(mode, rk);
+    if constexpr (sizeof(TI) == 4 && sizeof(TO) == 4) {
+        if (mode == 1)
+            return rk == 0 ? spmm_csr_kernel<TI, TO, VEC, G, ITERS, 1, 0>
+                           : spmm_csr_kernel<TI, TO, VEC, G, ITERS, 1, 1>;
+        return rk == 0 ? spmm_csr_kernel<TI, TO, VEC, G, ITERS, 0, 0> : spmm_csr_kernel<TI, TO, VEC, G, ITERS, 0, 1>;
+    } else if constexpr (VEC == 4 && ITERS == 2) {
+        return rk == 0 ? spmm_csr_capped_kernel<TI, TO, VEC, G, ITERS, 0>
+                       : spmm_csr_capped_kernel<TI, TO, VEC, G, ITERS, 1>;
+    } else {
+        return rk == 0 ? spmm_csr_kernel<TI, TO, VEC, G, ITERS, 0, 0> : spmm_csr_kernel<TI, TO, VEC, G, ITERS, 0, 1>;
     }
 }
 
-static SpmmKernel pick_kernel(const Shape &s, int mode, int rk) {
-    return s.vec == 4 ? pick_kernel_v<4>(s, mode, rk) : pick_kernel_v<1>(s, mode, rk);
-}
-
-template <typename TI, typename TO, int VEC, int G, int ITERS>
-static SpmmKernel pick_rk_x16(int rk) {
-    if constexpr (x16_capped<VEC, ITERS>())
-        return rk == 0 ? spmm_csr_x16_capped_kernel<TI, TO, VEC, G, ITERS, 0>
-                       : spmm_csr_x16_capped_kernel<TI, TO, VEC, G, ITERS, 1>;
-    else
-        return rk == 0 ? spmm_csr_x16_kernel<TI, TO, VEC, G, ITERS, 0> : spmm_csr_x16_kernel<TI, TO, VEC, G, ITERS, 1>;
-}
-
 template <typename TI, typename TO, int VEC>
-static SpmmKernel pick_kernel_x16_v(const Shape &s, int rk) {
+static SpmmKernel pick_kernel_v(const Shape &s, int mode, int rk) {
     switch (s.g) {
-        case 4: return pick_rk_x16<TI, TO, VEC, 4, 1>(rk);
-        case 8: return pick_rk_x16<TI, TO, VEC, 8, 1>(rk);
-        case 16: return pick_rk_x16<TI, TO, VEC, 16, 1>(rk);
+        case 4: return pick_mode<TI, TO, VEC, 4, 1>(mode, rk);
+        case 8: return pick_mode<TI, TO, VEC, 8, 1>(mode, rk);
+        case 16: return pick_mode<TI, TO, VEC, 16, 1>(mode, rk);
         default:
-            if (s.iters == 1) return pick_rk_x16<TI, TO, VEC, 32, 1>(rk);
-            if (s.iters == 2) return pick_rk_x16<TI, TO, VEC, 32, 2>(rk);
-            return pick_rk_x16<TI, TO, VEC, 32, 4>(rk);
+            if (s.iters == 1) return pick_mode<TI, TO, VEC, 32, 1>(mode, rk);
+            if (s.iters == 2) return pick_mode<TI, TO, VEC, 32, 2>(mode, rk);
+            return pick_mode<TI, TO, VEC, 32, 4>(mode, rk);
     }
 }
 
 template <typename TI, typename TO>
-static SpmmKernel pick_kernel_x16(const Shape &s, int rk) {
-    return s.vec == 4 ? pick_kernel_x16_v<TI, TO, 4>(s, rk) : pick_kernel_x16_v<TI, TO, 1>(s, rk);
+static SpmmKernel pick_kernel(const Shape &s, int mode, int rk) {
+    return s.vec == 4 ? pick_kernel_v<TI, TO, 4>(s, mode, rk) : pick_kernel_v<TI, TO, 1>(s, mode, rk);
 }
 
 struct HubWs {
@@ -484,7 +463,7 @@ static inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t
 size_t stream_ws_bytes(int64_t E, int64_t D);
 int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, int64_t ldx,
                     float *out, int64_t ldo, int64_t n_dst, int64_t n_src, int64_t E, int64_t D,
-                    int reduce_op, const float *scale_src, const float *scale_slot, const float *scale_dst,
+                    int reduce_op, const float *scale_src, const float *scale_dst,
                     const uint32_t *cols32, int l2_hints, int accumulate, const int64_t *eid,
                     const float *y, int64_t ldy, int y_bcast, int head_dim, int msg_op, void *ws,
                     size_t ws_bytes, cudaStream_t stream);
@@ -494,24 +473,28 @@ int gat_fused_run(const int64_t *indptr, const int64_t *cols, const float *f, in
                   const float *attn_src, const float *attn_dst, float slope, float *lse, void *ws, size_t ws_bytes,
                   cudaStream_t stream);
 
-// spmm_v5_kernel over 16-bit rows (copy sum / mean, 64 < D <= 128, D % 8 == 0): whether it takes a call, and the run
-bool stream_x16_eligible(const int64_t *cols, const uint32_t *cols32, const void *x, int64_t ldx, const void *out,
-                         int64_t ldo, int64_t n_src, int64_t E, int64_t D, int reduce_op);
-int spmm_stream_run_x16(int dtype, const int64_t *indptr, const int64_t *cols, const void *x, int64_t ldx, void *out,
-                        int64_t ldo, int64_t n_dst, int64_t E, int64_t D, int reduce_op,
-                        const float *scale_src, const float *scale_slot, const float *scale_dst, const uint32_t *cols32,
-                        int l2_hints, void *ws, size_t ws_bytes, cudaStream_t stream);
+// spmm_v5_kernel over rows of element type T (float, __nv_bfloat16 or __half): whether it takes a call, and the run
+template <typename T>
+bool v5_eligible(const int64_t *cols, const uint32_t *cols32, const void *x, int64_t ldx, const void *out, int64_t ldo,
+                 int64_t n_src, int64_t E, int64_t D, int reduce_op);
+template <typename T>
+int spmm_v5_run(const int64_t *indptr, const int64_t *cols, const void *x, int64_t ldx, void *out, int64_t ldo,
+                int64_t n_dst, int64_t E, int64_t D, int reduce_op, const float *scale_src, const float *scale_slot,
+                const float *scale_dst, const uint32_t *cols32, int l2_hints, int accumulate, void *ws,
+                size_t ws_bytes, cudaStream_t stream);
 
 // The node-parallel launch sequence behind both entries: spmm_csr kernel over all rows, then, when some row is longer
-// than HUB_T slots, the hub plan and the two hub passes.  x / out are float, or 16-bit for pglb_spmm_csr_x16.
-// k_main runs over the rows, k_chunk turns hub chunks into fp32 partials, k_merge reduces a hub's partials into its row.
+// than HUB_T slots, the hub plan and the two hub passes.  E is the element type of x and out.  The main pass reads E
+// and writes E, hub pass 1 turns chunks into fp32 partials, and pass 2 reduces a hub's partials into its E row.
+template <typename E>
 static int spmm_generic_run(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const void *x,
                             int64_t ldx, const float *y, int64_t ldy, int y_bcast, void *out, int64_t ldo,
                             int64_t n_dst, int64_t num_edges, int64_t D, int64_t head_dim, int msg_op, int reduce_op,
                             const float *scale_src, const float *scale_dst, int64_t max_degree_hint, int accumulate,
-                            const Shape &s, SpmmKernel k_main, SpmmKernel k_chunk, SpmmKernel k_merge, void *ws,
-                            size_t ws_bytes, cudaStream_t stream) {
-
+                            bool vec4, void *ws, size_t ws_bytes, cudaStream_t stream) {
+    const Shape s = pick_shape(D, vec4);
+    const int mode = (msg_op == PGLB_MSG_COPY) ? 0 : 1;
+    const int rk = (reduce_op >= PGLB_REDUCE_MAX) ? 1 : 0;
     const bool need_hub = !(max_degree_hint >= 0 && max_degree_hint <= HUB_T) && num_edges > HUB_T;
     HubWs h{};
     if (need_hub) {
@@ -559,7 +542,7 @@ static int spmm_generic_run(const int64_t *indptr, const int64_t *cols, const in
         const int64_t blocks = (tasks + gpb - 1) / gpb;
         PGLB_CHECK_ARG(blocks <= 0x7fffffffLL, PGLB_ESHAPE, "pglb_spmm_csr: grid too large");
         dim3 grid((unsigned)blocks, (unsigned)s.tiles);
-        k_main<<<grid, kThreads, 0, stream>>>(p);
+        pick_kernel<E, E>(s, mode, rk)<<<grid, kThreads, 0, stream>>>(p);
         PGLB_LAUNCH_CHECK("spmm_csr_kernel");
     }
     if (need_hub) {
@@ -586,7 +569,7 @@ static int spmm_generic_run(const int64_t *indptr, const int64_t *cols, const in
             if (blocks > max_blocks) blocks = max_blocks;
             // partial rows are dpad floats, 16-byte aligned => same vector shape is valid
             dim3 grid((unsigned)blocks, (unsigned)s.tiles);
-            k_chunk<<<grid, kThreads, 0, stream>>>(p1);
+            pick_kernel<E, float>(s, mode, rk)<<<grid, kThreads, 0, stream>>>(p1);
             PGLB_LAUNCH_CHECK("spmm_csr_kernel(hub pass 1)");
         }
         // pass 2: partials of a hub -> its output row
@@ -611,7 +594,7 @@ static int spmm_generic_run(const int64_t *indptr, const int64_t *cols, const in
             int64_t blocks = (h.hub_cap + gpb - 1) / gpb;
             if (blocks > max_blocks) blocks = max_blocks;
             dim3 grid((unsigned)blocks, (unsigned)s.tiles);
-            k_merge<<<grid, kThreads, 0, stream>>>(p2);
+            pick_kernel<float, E>(s, 0, rk)<<<grid, kThreads, 0, stream>>>(p2);
             PGLB_LAUNCH_CHECK("spmm_csr_kernel(hub pass 2)");
         }
     }
@@ -645,6 +628,21 @@ extern "C" int pglb_spmm_csr_f32(const int64_t *indptr, const int64_t *cols, con
                                         max_degree_hint, flags, ws, ws_bytes, stream_);
 }
 
+// The argument checks both spmm entries make; `entry` names the caller in pglb_last_error().  A call without work
+// (n_dst or D is 0) passes without the pointer and shape checks, so the caller's own early-out follows this call.
+static int spmm_check_args(const char *entry, const int64_t *indptr, const void *x, int64_t ldx, const void *out,
+                           int64_t ldo, int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t D, int reduce_op) {
+    PGLB_CHECK_ARG(n_dst >= 0 && n_src >= 0 && num_edges >= 0 && D >= 0, PGLB_EINVAL, "%s: negative size", entry);
+    PGLB_CHECK_ARG(reduce_op >= PGLB_REDUCE_SUM && reduce_op <= PGLB_REDUCE_MIN, PGLB_EINVAL,
+                   "%s: unknown reduce_op %d", entry, reduce_op);
+    if (n_dst == 0 || D == 0) return PGLB_OK;
+    PGLB_CHECK_ARG(indptr && out, PGLB_EINVAL, "%s: indptr/out is NULL", entry);
+    PGLB_CHECK_ARG(num_edges == 0 || x, PGLB_EINVAL, "%s: x is NULL", entry);
+    PGLB_CHECK_ARG(ldx >= D && ldo >= D, PGLB_ESHAPE, "%s: leading dimension smaller than D", entry);
+    PGLB_CHECK_ARG(D <= INT32_MAX, PGLB_ESHAPE, "%s: D too large", entry);
+    return PGLB_OK;
+}
+
 extern "C" int pglb_spmm_csr_slot_scale_f32(const int64_t *indptr, const int64_t *cols, const int64_t *eid,
                                             const float *x, int64_t ldx, const float *y, int64_t ldy,
                                             int y_bcast, float *out, int64_t ldo, int64_t n_dst,
@@ -654,19 +652,15 @@ extern "C" int pglb_spmm_csr_slot_scale_f32(const int64_t *indptr, const int64_t
                                             const uint32_t *cols_packed, int64_t max_degree_hint, int flags,
                                             void *ws, size_t ws_bytes, void *stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    PGLB_CHECK_ARG(n_dst >= 0 && n_src >= 0 && num_edges >= 0 && D >= 0, PGLB_EINVAL,
-                   "pglb_spmm_csr_f32: negative size");
-    PGLB_CHECK_ARG(reduce_op >= PGLB_REDUCE_SUM && reduce_op <= PGLB_REDUCE_MIN, PGLB_EINVAL,
-                   "pglb_spmm_csr_f32: unknown reduce_op %d", reduce_op);
     PGLB_CHECK_ARG(msg_op >= PGLB_MSG_COPY && msg_op <= PGLB_MSG_DIV, PGLB_EINVAL,
                    "pglb_spmm_csr_f32: unknown msg_op %d", msg_op);
     PGLB_CHECK_ARG(!scale_slot || scale_src, PGLB_EINVAL, "pglb_spmm_csr_slot_scale_f32: scale_slot needs scale_src");
+    {
+        const int rc = spmm_check_args("pglb_spmm_csr_f32", indptr, x, ldx, out, ldo, n_dst, n_src, num_edges, D,
+                                       reduce_op);
+        if (rc) return rc;
+    }
     if (n_dst == 0 || D == 0) return PGLB_OK;
-    PGLB_CHECK_ARG(indptr && out, PGLB_EINVAL, "pglb_spmm_csr_f32: indptr/out is NULL");
-    PGLB_CHECK_ARG(num_edges == 0 || x, PGLB_EINVAL, "pglb_spmm_csr_f32: x is NULL");
-    PGLB_CHECK_ARG(ldx >= D && ldo >= D, PGLB_ESHAPE,
-                   "pglb_spmm_csr_f32: leading dimension smaller than D");
-    PGLB_CHECK_ARG(D <= INT32_MAX, PGLB_ESHAPE, "pglb_spmm_csr_f32: D too large");
     const int accumulate = (flags & PGLB_SPMM_ACCUMULATE) ? 1 : 0;
     PGLB_CHECK_ARG(!accumulate || reduce_op == PGLB_REDUCE_SUM, PGLB_EUNSUPPORTED,
                    "pglb_spmm_csr_f32: PGLB_SPMM_ACCUMULATE needs reduce_op SUM");
@@ -682,7 +676,7 @@ extern "C" int pglb_spmm_csr_slot_scale_f32(const int64_t *indptr, const int64_t
     const bool vec4 = (D % 4 == 0) && (ldx % 4 == 0) && (ldo % 4 == 0) && aligned16(x) &&
                       aligned16(out) &&
                       (mode == 0 || y_bcast != PGLB_BCAST_FULL || ((ldy % 4 == 0) && aligned16(y)));
-    // wide rows: the edge-balanced cp.async-ring kernels (spmm_stream.cu).  With an edge operand
+    // wide rows: the edge-balanced kernels (spmm_stream.cu), spmm_v5_kernel where it applies.  With an edge operand
     // only the GAT shape qualifies: per-head (head_dim % 4 == 0) or scalar y, mul / add, D <= 128.
     const bool ue_fast = mode == 1 && D <= 128 && scale_src == nullptr && num_edges < 0x7fffffffLL &&
                          (msg_op == PGLB_MSG_MUL || msg_op == PGLB_MSG_ADD) &&
@@ -690,17 +684,17 @@ extern "C" int pglb_spmm_csr_slot_scale_f32(const int64_t *indptr, const int64_t
     if ((mode == 0 || ue_fast) && vec4 && D > 64 && num_edges > 0) {
         PGLB_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
                        "pglb_spmm_csr_f32: workspace must be 256-byte aligned");
-        return spmm_stream_run(indptr, cols, x, ldx, out, ldo, n_dst, n_src, num_edges, D,
-                               reduce_op, scale_src, scale_slot, scale_dst, mode == 0 ? cols_packed : nullptr,
-                               (flags & PGLB_SPMM_L2_HINTS) ? 1 : 0, accumulate, eid,
-                               mode == 1 ? y : nullptr, ldy, y_bcast, (int)head_dim, msg_op, ws,
-                               ws_bytes, stream);
+        const int l2_hints = (flags & PGLB_SPMM_L2_HINTS) ? 1 : 0;
+        if (mode == 0 && v5_eligible<float>(cols, cols_packed, x, ldx, out, ldo, n_src, num_edges, D, reduce_op))
+            return spmm_v5_run<float>(indptr, cols, x, ldx, out, ldo, n_dst, num_edges, D, reduce_op, scale_src,
+                                      scale_slot, scale_dst, cols_packed, l2_hints, accumulate, ws, ws_bytes, stream);
+        return spmm_stream_run(indptr, cols, x, ldx, out, ldo, n_dst, n_src, num_edges, D, reduce_op, scale_src,
+                               scale_dst, mode == 0 ? cols_packed : nullptr, l2_hints, accumulate, eid,
+                               mode == 1 ? y : nullptr, ldy, y_bcast, (int)head_dim, msg_op, ws, ws_bytes, stream);
     }
-    const Shape s = pick_shape(D, vec4);
-    const int rk = (reduce_op >= PGLB_REDUCE_MAX) ? 1 : 0;
-    return spmm_generic_run(indptr, cols, eid, x, ldx, y, ldy, y_bcast, out, ldo, n_dst, num_edges, D, head_dim, msg_op,
-                            reduce_op, scale_src, scale_dst, max_degree_hint, accumulate, s, pick_kernel(s, mode, rk),
-                            pick_kernel(s, mode, rk), pick_kernel(s, 0, rk), ws, ws_bytes, stream);
+    return spmm_generic_run<float>(indptr, cols, eid, x, ldx, y, ldy, y_bcast, out, ldo, n_dst, num_edges, D, head_dim,
+                                   msg_op, reduce_op, scale_src, scale_dst, max_degree_hint, accumulate, vec4, ws,
+                                   ws_bytes, stream);
 }
 
 extern "C" int pglb_spmm_csr_x16(const int64_t *indptr, const int64_t *cols, const void *x, int64_t ldx, void *out,
@@ -711,40 +705,32 @@ extern "C" int pglb_spmm_csr_x16(const int64_t *indptr, const int64_t *cols, con
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL,
                    "pglb_spmm_csr_x16: unknown dtype %d", dtype);
-    PGLB_CHECK_ARG(n_dst >= 0 && n_src >= 0 && num_edges >= 0 && D >= 0, PGLB_EINVAL,
-                   "pglb_spmm_csr_x16: negative size");
-    PGLB_CHECK_ARG(reduce_op >= PGLB_REDUCE_SUM && reduce_op <= PGLB_REDUCE_MIN, PGLB_EINVAL,
-                   "pglb_spmm_csr_x16: unknown reduce_op %d", reduce_op);
     PGLB_CHECK_ARG(!scale_slot || scale_src, PGLB_EINVAL, "pglb_spmm_csr_x16: scale_slot needs scale_src");
     PGLB_CHECK_ARG(!(flags & PGLB_SPMM_ACCUMULATE), PGLB_EUNSUPPORTED,
                    "pglb_spmm_csr_x16: PGLB_SPMM_ACCUMULATE would round the output twice");
-    if (n_dst == 0 || D == 0) return PGLB_OK;
-    PGLB_CHECK_ARG(indptr && out, PGLB_EINVAL, "pglb_spmm_csr_x16: indptr/out is NULL");
-    PGLB_CHECK_ARG(num_edges == 0 || x, PGLB_EINVAL, "pglb_spmm_csr_x16: x is NULL");
-    PGLB_CHECK_ARG(ldx >= D && ldo >= D, PGLB_ESHAPE, "pglb_spmm_csr_x16: leading dimension smaller than D");
-    PGLB_CHECK_ARG(D <= INT32_MAX, PGLB_ESHAPE, "pglb_spmm_csr_x16: D too large");
-    if (num_edges > 0 && stream_x16_eligible(cols, cols_packed, x, ldx, out, ldo, n_src, num_edges, D, reduce_op)) {
-        PGLB_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
-                       "pglb_spmm_csr_x16: workspace must be 256-byte aligned");
-        return spmm_stream_run_x16(dtype, indptr, cols, x, ldx, out, ldo, n_dst, num_edges, D, reduce_op,
-                                   scale_src, scale_slot, scale_dst, cols_packed,
-                                   (flags & PGLB_SPMM_L2_HINTS) ? 1 : 0, ws, ws_bytes, stream);
+    {
+        const int rc = spmm_check_args("pglb_spmm_csr_x16", indptr, x, ldx, out, ldo, n_dst, n_src, num_edges, D,
+                                       reduce_op);
+        if (rc) return rc;
     }
-    // every other shape: the node-parallel kernel, 8 bytes (4 elements) per lane when rows allow it
-    auto aligned8 = [](const void *q) { return (reinterpret_cast<uintptr_t>(q) & 7u) == 0; };
-    const bool vec4 = (D % 4 == 0) && (ldx % 4 == 0) && (ldo % 4 == 0) && aligned8(x) && aligned8(out);
-    const Shape s = pick_shape(D, vec4);
-    const int rk = (reduce_op >= PGLB_REDUCE_MAX) ? 1 : 0;
-    if (dtype == PGLB_DTYPE_BF16)
-        return spmm_generic_run(indptr, cols, nullptr, x, ldx, nullptr, 0, 0, out, ldo, n_dst, num_edges, D, 1,
-                                PGLB_MSG_COPY, reduce_op, scale_src, scale_dst, max_degree_hint, 0, s,
-                                pick_kernel_x16<__nv_bfloat16, __nv_bfloat16>(s, rk),
-                                pick_kernel_x16<__nv_bfloat16, float>(s, rk),
-                                pick_kernel_x16<float, __nv_bfloat16>(s, rk), ws, ws_bytes, stream);
-    return spmm_generic_run(indptr, cols, nullptr, x, ldx, nullptr, 0, 0, out, ldo, n_dst, num_edges, D, 1,
-                            PGLB_MSG_COPY, reduce_op, scale_src, scale_dst, max_degree_hint, 0, s,
-                            pick_kernel_x16<__half, __half>(s, rk), pick_kernel_x16<__half, float>(s, rk),
-                            pick_kernel_x16<float, __half>(s, rk), ws, ws_bytes, stream);
+    if (n_dst == 0 || D == 0) return PGLB_OK;
+    auto run = [&](auto *elem) -> int {
+        using T = std::remove_pointer_t<decltype(elem)>;
+        if (num_edges > 0 && v5_eligible<T>(cols, cols_packed, x, ldx, out, ldo, n_src, num_edges, D, reduce_op)) {
+            PGLB_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
+                           "pglb_spmm_csr_x16: workspace must be 256-byte aligned");
+            return spmm_v5_run<T>(indptr, cols, x, ldx, out, ldo, n_dst, num_edges, D, reduce_op, scale_src, scale_slot,
+                                  scale_dst, cols_packed, (flags & PGLB_SPMM_L2_HINTS) ? 1 : 0, 0, ws, ws_bytes,
+                                  stream);
+        }
+        // every other shape: the node-parallel kernel, 8 bytes (4 elements) per lane when rows allow it
+        auto aligned8 = [](const void *q) { return (reinterpret_cast<uintptr_t>(q) & 7u) == 0; };
+        const bool vec4 = (D % 4 == 0) && (ldx % 4 == 0) && (ldo % 4 == 0) && aligned8(x) && aligned8(out);
+        return spmm_generic_run<T>(indptr, cols, nullptr, x, ldx, nullptr, 0, 0, out, ldo, n_dst, num_edges, D, 1,
+                                   PGLB_MSG_COPY, reduce_op, scale_src, scale_dst, max_degree_hint, 0, vec4, ws,
+                                   ws_bytes, stream);
+    };
+    return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
 }
 
 static int gat_fused_entry(const char *name, const int64_t *indptr, const int64_t *cols, const float *f, int64_t ldf,

@@ -31,12 +31,11 @@ namespace pglb {
 constexpr int RING = 32;  // slots per lane ring == one column batch
 constexpr int GRP = 8;    // rows per cp.async commit group
 constexpr int LAG = 3;    // groups in flight behind the issue point
-constexpr int SW = 7;     // warps per block (7 * 16 KB = 112 KB smem, two blocks per SM)
 
 struct StreamP {
     const int64_t *indptr;
     const int64_t *cols;  // nullable: identity
-    const float *x;  // x / out: float, or the 16-bit element type of the *_x16 kernels (ldx / ldo in elements)
+    const float *x;  // x / out: float, or the 16-bit element type T of spmm_v5_kernel<T, ...> (ldx / ldo in elements)
     int64_t ldx;
     float *out;
     int64_t ldo;
@@ -693,7 +692,7 @@ __global__ void __launch_bounds__(StreamCfg<ITERS>::kThreads) spmm_stream_kernel
 // One warp per task that owns a cut row: out[r] = epilogue(tail(t) (+) head(t+1) (+) ...).  The partials are fp32;
 // TO is the element type of out (a 16-bit out is rounded once, on the store).
 template <typename TO, int ITERS, int RK>
-__device__ __forceinline__ void spmm_stream_fixup_body(const StreamP &p) {
+__global__ void __launch_bounds__(256) spmm_stream_fixup_kernel(const StreamP p) {
     const int lane = threadIdx.x & 31;
     const int64_t t = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (t >= p.ntasks) return;
@@ -755,15 +754,6 @@ __device__ __forceinline__ void spmm_stream_fixup_body(const StreamP &p) {
     }
 }
 
-template <int ITERS, int RK>
-__global__ void __launch_bounds__(256) spmm_stream_fixup_kernel(const StreamP p) {
-    spmm_stream_fixup_body<float, ITERS, RK>(p);
-}
-template <typename T>
-__global__ void __launch_bounds__(256) spmm_stream_fixup_x16_kernel(const StreamP p) {
-    spmm_stream_fixup_body<T, 1, 0>(p);
-}
-
 // Fused-GAT fix-up: merge the (acc, m, l) partials of a cut row: M = max m_i,
 // out = sum_i acc_i e^{m_i - M} / sum_i l_i e^{m_i - M}
 __global__ void __launch_bounds__(256) spmm_stream_fixup_gat_kernel(const StreamP p) {
@@ -799,9 +789,9 @@ __global__ void __launch_bounds__(256) spmm_stream_fixup_gat_kernel(const Stream
 // rows at a time; the streaming tasks above never touch empty rows.  TO: element type of out (16-bit: D % 4 == 0,
 // rows 8-byte aligned, never accumulating).
 template <typename TO>
-__device__ __forceinline__ void empty_rows_body(const int64_t *__restrict__ indptr, int64_t n_rows, int D,
-                                                float *__restrict__ out, int64_t ldo,
-                                                const float *__restrict__ scale_dst, int accumulate) {
+__global__ void __launch_bounds__(256) empty_rows_kernel(const int64_t *__restrict__ indptr, int64_t n_rows, int D,
+                                                         float *__restrict__ out, int64_t ldo,
+                                                         const float *__restrict__ scale_dst, int accumulate) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -833,26 +823,15 @@ __device__ __forceinline__ void empty_rows_body(const int64_t *__restrict__ indp
     }
 }
 
-__global__ void __launch_bounds__(256) empty_rows_kernel(const int64_t *__restrict__ indptr,
-                                                         int64_t n_rows, int D, float *__restrict__ out,
-                                                         int64_t ldo, const float *__restrict__ scale_dst,
-                                                         int accumulate) {
-    empty_rows_body<float>(indptr, n_rows, D, out, ldo, scale_dst, accumulate);
-}
-template <typename T>
-__global__ void __launch_bounds__(256) empty_rows_x16_kernel(const int64_t *__restrict__ indptr, int64_t n_rows, int D,
-                                                             float *__restrict__ out, int64_t ldo) {
-    empty_rows_body<T>(indptr, n_rows, D, out, ldo, nullptr, 0);
-}
-
+template <typename TO>
 static int launch_empty_rows(const StreamP &p, cudaStream_t stream) {
     if (p.accumulate && !p.scale_dst) return PGLB_OK;  // out_prev + 0 unchanged
     int64_t blocks = (p.n_rows + 255) / 256;
     const int64_t cap = (int64_t)sm_count() * 8;
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
-    empty_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(p.indptr, p.n_rows, p.D, p.out, p.ldo,
-                                                           p.scale_dst, p.accumulate);
+    empty_rows_kernel<TO><<<(unsigned)blocks, 256, 0, stream>>>(p.indptr, p.n_rows, p.D, p.out, p.ldo,
+                                                               p.scale_dst, p.accumulate);
     PGLB_LAUNCH_CHECK("empty_rows_kernel");
     return PGLB_OK;
 }
@@ -976,7 +955,7 @@ static int launch_stream128(const StreamP &p, cudaStream_t stream) {
     if (YM == 2) {
         spmm_stream_fixup_gat_kernel<<<(unsigned)fblocks, 256, 0, stream>>>(p);
     } else {
-        spmm_stream_fixup_kernel<1, RK><<<(unsigned)fblocks, 256, 0, stream>>>(p);
+        spmm_stream_fixup_kernel<float, 1, RK><<<(unsigned)fblocks, 256, 0, stream>>>(p);
     }
     PGLB_LAUNCH_CHECK("spmm_stream_fixup_kernel");
     return PGLB_OK;
@@ -994,18 +973,18 @@ static int launch_stream(const StreamP &p, int tiles, cudaStream_t stream) {
     PGLB_LAUNCH_CHECK("spmm_stream_kernel");
     const int64_t fblocks = (p.ntasks * 32 + 255) / 256;
     dim3 fgrid((unsigned)fblocks, (unsigned)tiles);
-    spmm_stream_fixup_kernel<ITERS, RK><<<fgrid, 256, 0, stream>>>(p);
+    spmm_stream_fixup_kernel<float, ITERS, RK><<<fgrid, 256, 0, stream>>>(p);
     PGLB_LAUNCH_CHECK("spmm_stream_fixup_kernel");
     return PGLB_OK;
 }
 
-// Task plan and launch parameters shared by the wide-row runs below; fills everything of p but the edge operand and
-// accumulate (left as the caller set them).  `ws` holds >= stream_ws_bytes().
-static int stream_prepare(StreamP &p, const int64_t *indptr, const int64_t *cols, const void *x, int64_t ldx,
+// Task plan and launch parameters shared by the wide-row runs below: fills everything of p but the edge operand,
+// accumulate and the task hand-out p.dyn (left to the caller), and launches task_plan_kernel for tasks of T slots.
+// `ws` holds >= stream_ws_bytes().
+static int stream_prepare(StreamP &p, int64_t T, const int64_t *indptr, const int64_t *cols, const void *x, int64_t ldx,
                           void *out, int64_t ldo, int64_t n_dst, int64_t E, int64_t D, int reduce_op,
                           const float *scale_src, const float *scale_slot, const float *scale_dst,
                           const uint32_t *cols32, void *ws, size_t ws_bytes, cudaStream_t stream) {
-    const int64_t T = stream_task_size(E);
     PGLB_CHECK_ARG(E > 0, PGLB_EINVAL, "spmm_stream_run: needs at least one slot");
     StreamWs w = stream_layout(ws, E, D, T);
     PGLB_CHECK_ARG(ws != nullptr && ws_bytes >= w.bytes, PGLB_EWORKSPACE,
@@ -1022,17 +1001,17 @@ static int stream_prepare(StreamP &p, const int64_t *indptr, const int64_t *cols
     p.reduce_op = reduce_op;
     p.scale_src = scale_src;
     p.scale_dst = scale_dst;
-    p.scale_slot = scale_slot;  // spmm_v5 only; the other kernels below gather scale_src
+    p.scale_slot = scale_slot;  // spmm_v5 only; the other kernels gather scale_src
     p.T = T;
     p.ntasks = w.ntasks;
     p.first_row = w.first_row;
     p.start = w.start;
     p.partial = w.partial;
+    p.partial_ml = w.partial_ml;
     p.dpad = w.dpad;
     p.tail_row = w.tail_row;
     p.cols32 = cols32;
     p.counter = w.counter;
-    p.dyn = dyn_mode("PGLB_V5_DYN", 0, w.ntasks);
     p.trace = trace_for(w.ntasks);
     {
         const int64_t blocks = (w.ntasks + 1 + 255) / 256;
@@ -1043,10 +1022,42 @@ static int stream_prepare(StreamP &p, const int64_t *indptr, const int64_t *cols
     return PGLB_OK;
 }
 
-// Called by pglb_spmm_csr_f32 for the eligible shapes.  `ws` holds >= stream_ws_bytes().
+// Called by both spmm entries for the calls v5_eligible<T>() accepts; T is the element type of x and out.  `ws` holds
+// >= stream_ws_bytes().
+template <typename T>
+int spmm_v5_run(const int64_t *indptr, const int64_t *cols, const void *x, int64_t ldx, void *out, int64_t ldo,
+                int64_t n_dst, int64_t E, int64_t D, int reduce_op, const float *scale_src, const float *scale_slot,
+                const float *scale_dst, const uint32_t *cols32, int l2_hints, int accumulate, void *ws,
+                size_t ws_bytes, cudaStream_t stream) {
+    StreamP p{};
+    p.head_dim = 1;
+    p.accumulate = accumulate;
+    {
+        const int rc = stream_prepare(p, stream_task_size(E), indptr, cols, x, ldx, out, ldo, n_dst, E, D, reduce_op,
+                                      scale_src, scale_slot, scale_dst, cols32, ws, ws_bytes, stream);
+        if (rc) return rc;
+    }
+    p.dyn = dyn_mode("PGLB_V5_DYN", 0, p.ntasks);
+    {
+        const int rc = launch_empty_rows<T>(p, stream);
+        if (rc) return rc;
+    }
+    return launch_v5<T>(p, cols32 != nullptr && cols != nullptr && l2_hints != 0, stream);
+}
+
+// the instantiations the entries in spmm.cu call
+template decltype(v5_eligible<float>) v5_eligible<float>;
+template decltype(v5_eligible<__nv_bfloat16>) v5_eligible<__nv_bfloat16>;
+template decltype(v5_eligible<__half>) v5_eligible<__half>;
+template decltype(spmm_v5_run<float>) spmm_v5_run<float>;
+template decltype(spmm_v5_run<__nv_bfloat16>) spmm_v5_run<__nv_bfloat16>;
+template decltype(spmm_v5_run<__half>) spmm_v5_run<__half>;
+
+// Called by pglb_spmm_csr_f32 for the wide-row shapes spmm_v5_kernel does not take (max / min, edge operands, identity
+// columns).  `ws` holds >= stream_ws_bytes().
 int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, int64_t ldx,
                     float *out, int64_t ldo, int64_t n_dst, int64_t n_src, int64_t E, int64_t D,
-                    int reduce_op, const float *scale_src, const float *scale_slot, const float *scale_dst,
+                    int reduce_op, const float *scale_src, const float *scale_dst,
                     const uint32_t *cols32, int l2_hints, int accumulate, const int64_t *eid,
                     const float *y, int64_t ldy, int y_bcast, int head_dim, int msg_op, void *ws,
                     size_t ws_bytes, cudaStream_t stream) {
@@ -1059,20 +1070,18 @@ int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, 
     p.msg_op = msg_op;
     p.accumulate = accumulate;
     {
-        const int rc = stream_prepare(p, indptr, cols, x, ldx, out, ldo, n_dst, E, D, reduce_op, scale_src, scale_slot,
-                                      scale_dst, cols32, ws, ws_bytes, stream);
+        const int rc = stream_prepare(p, stream_task_size(E), indptr, cols, x, ldx, out, ldo, n_dst, E, D, reduce_op,
+                                      scale_src, nullptr, scale_dst, cols32, ws, ws_bytes, stream);
         if (rc) return rc;
     }
+    p.dyn = dyn_mode("PGLB_S128_DYN", 2, p.ntasks);   // round 1's kernel (max / min, edge operands): descending queue
     {
-        const int rc = launch_empty_rows(p, stream);
+        const int rc = launch_empty_rows<float>(p, stream);
         if (rc) return rc;
     }
     const int64_t cv = D / 4;
     const int rk = (reduce_op >= PGLB_REDUCE_MAX) ? 1 : 0;
     const bool small_ids = (cols ? n_src : E) < 0x7fffffffLL && ldx * 4 < 0xffffffffLL;
-    if (cv <= 32 && v5_eligible(p, n_src, rk, small_ids))
-        return launch_v5(p, cols32 != nullptr && cols != nullptr && l2_hints != 0, stream);
-    p.dyn = dyn_mode("PGLB_S128_DYN", 2, p.ntasks);   // round 1's kernel (max / min, edge operands): descending queue
     if (cv <= 32 && small_ids) {
         if (y) {  // edge operand: plain int64 ids, no source scale
             return rk ? launch_stream128<1, false, 0, 1>(p, stream) : launch_stream128<0, false, 0, 1>(p, stream);
@@ -1090,45 +1099,6 @@ int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, 
     if (iters == 2) return rk ? launch_stream<2, 1>(p, tiles, stream) : launch_stream<2, 0>(p, tiles, stream);
     return rk ? launch_stream<4, 1>(p, tiles, stream) : launch_stream<4, 0>(p, tiles, stream);
 }
-
-// spmm_v5_kernel over 16-bit rows: copy sum / mean, 64 < D <= 128, rows a multiple of 16 bytes (D % 8 == 0, as a bulk
-// copy needs), 16-byte aligned x and out, ids that fit the packed form.  Every other 16-bit call takes the node-parallel
-// kernel (spmm.cu).
-bool stream_x16_eligible(const int64_t *cols, const uint32_t *cols32, const void *x, int64_t ldx, const void *out,
-                         int64_t ldo, int64_t n_src, int64_t E, int64_t D, int reduce_op) {
-    if (reduce_op >= PGLB_REDUCE_MAX || D <= 64 || D > 128 || D % 8 != 0) return false;
-    if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(out) & 15) || ldx % 8 || ldo % 8)
-        return false;
-    if ((cols ? n_src : E) >= 0x7fffffffLL || ldx * 2 >= 0xffffffffLL) return false;  // small_ids of the fp32 run
-    if (v5_mode() == 1 && (n_src >= 0x7fffffffLL || (!cols && !cols32))) return false;  // as v5_eligible
-    return true;
-}
-
-template <typename T>
-static int run_x16(const StreamP &p, bool hot, cudaStream_t stream) {
-    int64_t blocks = (p.n_rows + 255) / 256;
-    const int64_t cap = (int64_t)sm_count() * 8;
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    empty_rows_x16_kernel<T><<<(unsigned)blocks, 256, 0, stream>>>(p.indptr, p.n_rows, p.D, p.out, p.ldo);
-    PGLB_LAUNCH_CHECK("empty_rows_kernel");
-    return launch_v5<T>(p, hot, stream);
-}
-
-// Called by pglb_spmm_csr_x16 when stream_x16_eligible().  `ws` holds >= stream_ws_bytes().
-int spmm_stream_run_x16(int dtype, const int64_t *indptr, const int64_t *cols, const void *x, int64_t ldx, void *out,
-                        int64_t ldo, int64_t n_dst, int64_t E, int64_t D, int reduce_op,
-                        const float *scale_src, const float *scale_slot, const float *scale_dst, const uint32_t *cols32,
-                        int l2_hints, void *ws, size_t ws_bytes, cudaStream_t stream) {
-    StreamP p{};
-    p.head_dim = 1;
-    const int rc = stream_prepare(p, indptr, cols, x, ldx, out, ldo, n_dst, E, D, reduce_op, scale_src, scale_slot,
-                                  scale_dst, cols32, ws, ws_bytes, stream);
-    if (rc) return rc;
-    const bool hot = cols32 != nullptr && cols != nullptr && l2_hints != 0;
-    return dtype == PGLB_DTYPE_BF16 ? run_x16<__nv_bfloat16>(p, hot, stream) : run_x16<__half>(p, hot, stream);
-}
-
 
 // ---- narrow2 host side --------------------------------------------------------------------------------------
 // Slots per task of the narrow kernel: the wide kernel's choice rounded up to whole chunks of (32 / LPR) * 32 slots
@@ -1205,7 +1175,7 @@ int narrow2_run(const uint32_t *plan, const int32_t *nz_row, const int32_t *blk_
     sp.dpad = w.dpad;
     sp.tail_row = w.tail_row;
     {
-        const int rc = launch_empty_rows(sp, stream);
+        const int rc = launch_empty_rows<float>(sp, stream);
         if (rc) return rc;
     }
     const int64_t blocks = (p.ntasks + kNarrowWarps - 1) / kNarrowWarps;
@@ -1217,7 +1187,7 @@ int narrow2_run(const uint32_t *plan, const int32_t *nz_row, const int32_t *blk_
     else launch_narrow2<16>(p, sc, hot != 0, (unsigned)blocks, stream);
     PGLB_LAUNCH_CHECK("spmm_narrow2_kernel");
     const int64_t fblocks = (p.ntasks * 32 + 255) / 256;
-    spmm_stream_fixup_kernel<1, 0><<<(unsigned)fblocks, 256, 0, stream>>>(sp);
+    spmm_stream_fixup_kernel<float, 1, 0><<<(unsigned)fblocks, 256, 0, stream>>>(sp);
     PGLB_LAUNCH_CHECK("spmm_stream_fixup_kernel");
     return PGLB_OK;
 }
@@ -1227,54 +1197,29 @@ int gat_fused_run(const int64_t *indptr, const int64_t *cols, const float *f, in
                   int64_t ldo, int64_t n_dst, int64_t n_src, int64_t E, int64_t D, int64_t H,
                   const float *attn_src, const float *attn_dst, float slope, float *lse, void *ws, size_t ws_bytes,
                   cudaStream_t stream) {
-    const int64_t T = gat_task_size(E);
-    PGLB_CHECK_ARG(E > 0, PGLB_EINVAL, "gat_fused_run: needs at least one slot");
-    StreamWs w = stream_layout(ws, E, D, T);
-    PGLB_CHECK_ARG(ws != nullptr && ws_bytes >= w.bytes, PGLB_EWORKSPACE,
-                   "pglb_gat_fused_csr_f32: workspace of %zu bytes needed (got %zu)", w.bytes, ws_bytes);
+    // the row statistics are written by spmm_gat5_kernel and the merge kernel only
+    const bool tma = gat5_eligible(D, slope, f, ldf, attn_src, H, n_src);
+    PGLB_CHECK_ARG(!lse || tma, PGLB_EUNSUPPORTED,
+                   "pglb_gat_fused_train_csr_f32: shape outside the TMA kernel (H %% 4, 16-byte rows, 0 <= slope <= 1)");
     StreamP p{};
-    p.indptr = indptr;
-    p.cols = cols;
-    p.x = f;
-    p.ldx = ldf;
-    p.out = out;
-    p.ldo = ldo;
-    p.n_rows = n_dst;
-    p.E = E;
-    p.D = (int)D;
-    p.reduce_op = PGLB_REDUCE_SUM;
-    p.T = T;
-    p.ntasks = w.ntasks;
-    p.first_row = w.first_row;
-    p.start = w.start;
-    p.partial = w.partial;
-    p.partial_ml = w.partial_ml;
-    p.dpad = w.dpad;
-    p.tail_row = w.tail_row;
     p.y = attn_src;
     p.ldy = H;
     p.y_bcast = PGLB_BCAST_HEAD;
     p.head_dim = (int)(D / H);
     p.attn_dst = attn_dst;
     p.slope = slope;
-    p.counter = w.counter;
-    p.dyn = dyn_mode("PGLB_GAT_DYN", 1, w.ntasks);
-    p.trace = trace_for(w.ntasks);
     p.lse = lse;
-    // the row statistics are written by spmm_gat5_kernel and the merge kernel only
-    PGLB_CHECK_ARG(!lse || gat5_eligible(p, f, ldf, attn_src, H, n_src), PGLB_EUNSUPPORTED,
-                   "pglb_gat_fused_train_csr_f32: shape outside the TMA kernel (H %% 4, 16-byte rows, 0 <= slope <= 1)");
     {
-        const int64_t blocks = (w.ntasks + 1 + 255) / 256;
-        task_plan_kernel<<<(unsigned)blocks, 256, 0, stream>>>(indptr, n_dst, E, T, stream_snap(T),
-                                                               w.ntasks, w.first_row, w.start, w.counter);
-        PGLB_LAUNCH_CHECK("task_plan_kernel");
-    }
-    {
-        const int rc = launch_empty_rows(p, stream);
+        const int rc = stream_prepare(p, gat_task_size(E), indptr, cols, f, ldf, out, ldo, n_dst, E, D, PGLB_REDUCE_SUM,
+                                      nullptr, nullptr, nullptr, nullptr, ws, ws_bytes, stream);
         if (rc) return rc;
     }
-    if (gat5_eligible(p, f, ldf, attn_src, H, n_src)) return launch_gat5(p, attn_src, H, stream);
+    p.dyn = dyn_mode("PGLB_GAT_DYN", 1, p.ntasks);
+    {
+        const int rc = launch_empty_rows<float>(p, stream);
+        if (rc) return rc;
+    }
+    if (tma) return launch_gat5(p, attn_src, H, stream);
     return launch_stream128<0, false, 0, 2>(p, stream);
 }
 

@@ -289,6 +289,12 @@ def segment_indptr(segment_ids, num_segments):
 def _spmm_raw(indptr, cols, x2, n_dst, reduce_op, eid=None, y2=None, y_bcast=BCAST_FULL,
               head_dim=1, msg_op="copy", scale_src=None, scale_dst=None, max_degree=-1,
               num_edges=None, out=None, packed=None, accumulate=False):
+    """float32 x: pglb_spmm_csr_slot_scale_f32, or pglb_spmm_narrow_f32 with a NarrowPlan.  bfloat16 / float16 x:
+    copy messages only, through pglb_spmm_csr_x16.  The output has x's dtype."""
+    half = x2.dtype in HALF_DTYPES
+    if half and (msg_op != "copy" or y2 is not None or accumulate):
+        raise TypeError("pgl_b200: 16-bit features aggregate copy messages only (got msg_op=%s%s%s)"
+                        % (msg_op, ", an edge operand" if y2 is not None else "", ", accumulate" if accumulate else ""))
     dev = x2.device
     D = int(x2.shape[1])
     E = int(num_edges if num_edges is not None else (cols.shape[0] if cols is not None else 0))
@@ -297,14 +303,11 @@ def _spmm_raw(indptr, cols, x2, n_dst, reduce_op, eid=None, y2=None, y_bcast=BCA
         scale_src = scale_src.float()
     if scale_dst is not None and scale_dst.dtype != torch.float32:
         scale_dst = scale_dst.float()
-    if x2.dtype in HALF_DTYPES:
-        return _spmm_x16(indptr, cols, x2, n_dst, reduce_op, E, y2, msg_op, scale_src, scale_dst, max_degree, out,
-                         packed, accumulate)
     if out is None:
-        out = torch.empty((n_dst, D), dtype=torch.float32, device=dev)
+        out = torch.empty((n_dst, D), dtype=x2.dtype, device=dev)
     if isinstance(packed, NarrowPlan):
-        if (reduce_op in ("sum", "mean") and msg_op == "copy" and y2 is None and not accumulate and E > 0
-                and n_dst > 0 and x2.data_ptr() % 16 == 0 and x2.stride(0) % 4 == 0 and x2.stride(1) == 1
+        if (not half and reduce_op in ("sum", "mean") and msg_op == "copy" and y2 is None and not accumulate
+                and E > 0 and n_dst > 0 and x2.data_ptr() % 16 == 0 and x2.stride(0) % 4 == 0 and x2.stride(1) == 1
                 and out.data_ptr() % 16 == 0 and out.stride(0) % 4 == 0 and int(x2.shape[0]) < (1 << 30)):
             need = ctypes.c_size_t(0)
             check(lib.pglb_spmm_narrow_ws(E, D, ctypes.byref(need)))
@@ -323,47 +326,25 @@ def _spmm_raw(indptr, cols, x2, n_dst, reduce_op, eid=None, y2=None, y_bcast=BCA
     need = ctypes.c_size_t(0)
     check(lib.pglb_spmm_csr_ws(n_dst, E, D, ctypes.byref(need)))
     ws = workspace(dev, need.value)
-    wsn = ws.numel()
     sslot = None
     if (scale_src is not None and reduce_op in ("sum", "mean") and msg_op == "copy"
             and getattr(packed, "slot_scale", None) is not None):
         # scale_src[cols[j]] per slot (None before the scale's second call) for spmm_v5, the kernel of these calls
         sslot = packed.slot_scale(scale_src)
+    ids = _ptr(packed[0]) if packed is not None else None
+    flags = (1 if accumulate else 0) | (2 if (packed is not None and packed[1]) else 0)
     with torch.cuda.device(dev):
-        check(lib.pglb_spmm_csr_slot_scale_f32(
-            _ptr(indptr), _ptr(cols), _ptr(eid), _ptr(x2), x2.stride(0), _ptr(y2),
-            (y2.stride(0) if y2 is not None else 0), y_bcast, _ptr(out), out.stride(0), n_dst,
-            int(x2.shape[0]), E, D, head_dim, MSG[msg_op], REDUCE[reduce_op], _ptr(scale_src), _ptr(sslot),
-            _ptr(scale_dst), _ptr(packed[0]) if packed is not None else None, int(max_degree),
-            (1 if accumulate else 0) | (2 if (packed is not None and packed[1]) else 0), _ptr(ws),
-            wsn, _stream()))
-    return out
-
-
-def _spmm_x16(indptr, cols, x2, n_dst, reduce_op, E, y2, msg_op, scale_src, scale_dst, max_degree, out, packed,
-              accumulate):
-    """_spmm_raw for bfloat16 / float16 x: copy messages only, output in x's dtype (pglb_spmm_csr_x16)."""
-    if msg_op != "copy" or y2 is not None or accumulate:
-        raise TypeError("pgl_b200: 16-bit features aggregate copy messages only (got msg_op=%s%s%s)"
-                        % (msg_op, ", an edge operand" if y2 is not None else "", ", accumulate" if accumulate else ""))
-    dev = x2.device
-    D = int(x2.shape[1])
-    if out is None:
-        out = torch.empty((n_dst, D), dtype=x2.dtype, device=dev)
-    if isinstance(packed, NarrowPlan):
-        packed = None
-    need = ctypes.c_size_t(0)
-    check(lib.pglb_spmm_csr_ws(n_dst, E, D, ctypes.byref(need)))
-    ws = workspace(dev, need.value)
-    sslot = None
-    if scale_src is not None and reduce_op in ("sum", "mean") and getattr(packed, "slot_scale", None) is not None:
-        sslot = packed.slot_scale(scale_src)
-    with torch.cuda.device(dev):
-        check(lib.pglb_spmm_csr_x16(
-            _ptr(indptr), _ptr(cols), _ptr(x2), x2.stride(0), _ptr(out), out.stride(0), n_dst, int(x2.shape[0]), E, D,
-            _DTYPE16[x2.dtype], REDUCE[reduce_op], _ptr(scale_src), _ptr(sslot), _ptr(scale_dst),
-            _ptr(packed[0]) if packed is not None else None, int(max_degree),
-            2 if (packed is not None and packed[1]) else 0, _ptr(ws), ws.numel(), _stream()))
+        if half:
+            check(lib.pglb_spmm_csr_x16(
+                _ptr(indptr), _ptr(cols), _ptr(x2), x2.stride(0), _ptr(out), out.stride(0), n_dst, int(x2.shape[0]),
+                E, D, _DTYPE16[x2.dtype], REDUCE[reduce_op], _ptr(scale_src), _ptr(sslot), _ptr(scale_dst), ids,
+                int(max_degree), flags, _ptr(ws), ws.numel(), _stream()))
+        else:
+            check(lib.pglb_spmm_csr_slot_scale_f32(
+                _ptr(indptr), _ptr(cols), _ptr(eid), _ptr(x2), x2.stride(0), _ptr(y2),
+                (y2.stride(0) if y2 is not None else 0), y_bcast, _ptr(out), out.stride(0), n_dst,
+                int(x2.shape[0]), E, D, head_dim, MSG[msg_op], REDUCE[reduce_op], _ptr(scale_src), _ptr(sslot),
+                _ptr(scale_dst), ids, int(max_degree), flags, _ptr(ws), ws.numel(), _stream()))
     return out
 
 
@@ -699,26 +680,22 @@ def narrow_plan(indptr, cols, n_src, row_bytes=64):
 
 
 def _packed_of(csr, x2):
-    """Per-(graph, row width) index data from the EdgeIndex cache: packed column ids (+ optional L2 hints) for the
-    wide-row kernels (64 < D <= 128), the narrow plan for D <= 64.  16-bit rows: packed ids for the rows the wide-row
-    kernel takes (64 < D <= 128, D % 8 == 0), with the hot set chosen for their real size; None otherwise."""
+    """Per-(graph, row width) index data from the EdgeIndex cache: packed column ids (+ optional L2 hints, the hot set
+    chosen for the real row size) for the wide-row kernels (64 < D <= 128), the narrow plan for float32 rows of
+    D <= 64.  Only rows of at most 128 elements and a multiple of 16 bytes get either; the others get None."""
     fn = csr.get("packed")
     D = int(x2.shape[1])
-    if x2.dtype in HALF_DTYPES:
-        if fn is None or D > 128 or D <= 64 or D % 8:
-            return None
-        pk = fn(int(x2.shape[0]), D * x2.element_size())
-        return PackedCols(pk, csr.get("slot_scale")) if pk is not None else None
-    if fn is None or D > 128 or D % 4:
+    row_bytes = D * x2.element_size()
+    if fn is None or D > 128 or row_bytes % 16:
         return None
     n_src = int(x2.shape[0])
     if D <= 64:
-        if csr.get("plan") is not None and 0 < n_src < (1 << 30) and \
+        if x2.dtype == torch.float32 and csr.get("plan") is not None and 0 < n_src < (1 << 30) and \
                 csr["cols"] is not None and int(csr["cols"].shape[0]) > 0:
-            plan, nz_row, blk_k, hints = csr["plan"](n_src, D * 4)
+            plan, nz_row, blk_k, hints = csr["plan"](n_src, row_bytes)
             return NarrowPlan(plan, nz_row, blk_k, hints, slot_scale=csr.get("slot_scale"))
         return None
-    pk = fn(n_src, D * 4)
+    pk = fn(n_src, row_bytes)
     return PackedCols(pk, csr.get("slot_scale")) if pk is not None else None
 
 
