@@ -148,7 +148,7 @@ int pglb_spmm_csr_slot_scale_f32(const int64_t *indptr, const int64_t *cols, con
                                   another subset (halo rows) are still in flight */
 #define PGLB_SPMM_L2_HINTS 2   /* bit 31 of cols_packed carries an L2 residency hint */
 
-/* 16-bit feature types of pglb_spmm_csr_x16 */
+/* 16-bit feature types of pglb_spmm_csr_x16 and the other *_x16 entries */
 #define PGLB_DTYPE_BF16 1
 #define PGLB_DTYPE_F16 2
 /* Copy-message aggregation over 16-bit features: pglb_spmm_csr_slot_scale_f32 with msg_op = COPY (send_u_recv with
@@ -166,6 +166,21 @@ int pglb_spmm_csr_x16(const int64_t *indptr, const int64_t *cols, const void *x,
                       const float *scale_src, const float *scale_slot, const float *scale_dst,
                       const uint32_t *cols_packed, int64_t max_degree_hint, int flags, void *ws, size_t ws_bytes,
                       void *stream);
+
+/* Send/recv with an edge operand over 16-bit features: pglb_spmm_csr_f32's arguments plus `dtype`, x and out bfloat16
+ * or float16 (ldx / ldo in elements), y float32.  Instantiated for msg_op MUL / ADD, reduce_op SUM and y_bcast
+ * PGLB_BCAST_HEAD / PGLB_BCAST_SCALAR over rows of D % 4 == 0 elements (8-byte aligned x and out, ldx, ldo % 4 == 0):
+ * the gradient of the fused GAT aggregation wrt f, sum over the out-edges of alpha * grad_out[dst].  Any other msg_op,
+ * reduce_op or broadcast, D % 4 != 0 and PGLB_SPMM_ACCUMULATE are PGLB_EUNSUPPORTED; misaligned rows PGLB_ESHAPE.
+ * Numerics: each message x (op) y is formed and summed in fp32, in slot order, with the fp32 node-parallel kernel's
+ * operations; hub partials are fp32; each output is rounded once, to nearest even.  Deterministic.  Rows of up to 1024
+ * slots are summed sequentially.  cols_packed is not taken.  Unknown dtype: PGLB_EINVAL.  All argument checks precede
+ * any CUDA call.  ws: pglb_spmm_csr_ws(n_dst, E, D). */
+int pglb_spmm_csr_ue_x16(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const void *x, int64_t ldx,
+                         const float *y, int64_t ldy, int y_bcast, void *out, int64_t ldo, int64_t n_dst,
+                         int64_t n_src, int64_t num_edges, int64_t D, int64_t head_dim, int dtype, int msg_op,
+                         int reduce_op, const float *scale_src, const float *scale_dst, int64_t max_degree_hint,
+                         int flags, void *ws, size_t ws_bytes, void *stream);
 
 /* Packed column ids for pglb_spmm_csr_f32: count[n_src] (int32, zeroed by the call) receives how
  * often every source occurs in cols[E]; packed[j] = cols[j] | (count[cols[j]] >= min_count) << 31.
@@ -274,6 +289,11 @@ int pglb_gat_fused_csr_f32(const int64_t *indptr, const int64_t *cols, const flo
  * f rows of H*head_dim <= 128 floats, 16-byte aligned; head_dim in {4, 8, ..., 128}. */
 int pglb_head_dots_f32(const float *f, int64_t ldf, int64_t n, int64_t H, int64_t head_dim, const float *w_src,
                        const float *w_dst, float *attn_src, float *attn_dst, void *stream);
+/* The same over bfloat16 / float16 f (`dtype`, ldf in elements, rows 16-byte aligned); w_src, w_dst, attn_src and
+ * attn_dst are float32.  f is widened exactly and the products and adds are the fp32 entry's, in the same order: the
+ * result equals pglb_head_dots_f32 on the widened f bit for bit.  Unknown dtype: PGLB_EINVAL. */
+int pglb_head_dots_x16(const void *f, int64_t ldf, int64_t n, int64_t H, int64_t head_dim, int dtype,
+                       const float *w_src, const float *w_dst, float *attn_src, float *attn_dst, void *stream);
 
 /* Training forward of the same layer (GATConv under autograd, pgl/nn/conv.py:333-339; the reference gets the
  * backward from Paddle autograd over four ops): the same single launch, which also leaves
@@ -299,6 +319,40 @@ int pglb_gat_bwd_edge_f32(const int64_t *rows, const int64_t *cols, const int64_
                           const float *attn_src, const float *attn_dst, const float *lse,
                           float negative_slope, int64_t num_edges, int64_t H, int64_t head_dim,
                           float *alpha_e, float *dz_e, void *stream);
+
+/* The fused GAT aggregation over bfloat16 / float16 features (`dtype`): the fp32 entries' arguments, f and out in
+ * `dtype` (ldf / ldo in elements), attn_src, attn_dst and lse float32.
+ *   - Shapes: H % 4 == 0, H <= 32, D = H * head_dim <= 128 with D % 8 == 0, 0 <= slope <= 1, the kernel's
+ *     shared-memory budget, 16-byte aligned attn_src: otherwise PGLB_EUNSUPPORTED (there is no 16-bit fallback
+ *     kernel).  f and out 16-byte aligned with ldf, ldo % 8 == 0: otherwise PGLB_ESHAPE.
+ *   - Numerics: f is widened exactly; logits, LeakyReLU, the online softmax, rescales and accumulation are the fp32
+ *     kernel's instructions in the same slot order; cut-row partials and (m, l) are fp32; each output element is
+ *     rounded once, to nearest even.  So out == round16(pglb_gat_fused_csr_f32 on the widened f) bit for bit, and
+ *     the train entry's lse equals the fp32 train entry's lse bit for bit, for every shape both run on the TMA kernel.
+ *   - One shape only the 16-bit rings hold: H = 32 with head_dim = 4 (the halved feature rows leave room for 32
+ *     attention floats per row).  There the fp32 inference entry runs its per-slot kernel and the fp32 train entry
+ *     returns PGLB_EUNSUPPORTED, so nothing fp32 is bitwise comparable: out is within 2 u |ref32|_inf of the fp32
+ *     inference entry's output on the widened f (u = 2^-8 bf16, 2^-11 fp16), and lse within the path's 1e-4
+ *     relative bar of the exact log-sum-exp.
+ *   - Unknown dtype: PGLB_EINVAL; NULL lse on the train entry (n_dst > 0): PGLB_EINVAL.  All argument checks precede
+ *     any CUDA call.  ws as pglb_spmm_csr_ws(D = H*head_dim). */
+int pglb_gat_fused_csr_x16(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
+                           const float *attn_src, const float *attn_dst, float negative_slope, void *out,
+                           int64_t ldo, int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H, int64_t head_dim,
+                           int dtype, void *ws, size_t ws_bytes, void *stream);
+int pglb_gat_fused_train_csr_x16(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
+                                 const float *attn_src, const float *attn_dst, float negative_slope, void *out,
+                                 int64_t ldo, float *lse, int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H,
+                                 int64_t head_dim, int dtype, void *ws, size_t ws_bytes, void *stream);
+/* pglb_gat_bwd_edge_f32 over bfloat16 / float16 f, grad_out and out (`dtype`, rows 16-byte aligned, ld in elements);
+ * attn_src, attn_dst, lse, alpha_e and dz_e are float32.  The three row inputs are widened exactly and every value
+ * after that is the fp32 kernel's: alpha_e and dz_e equal pglb_gat_bwd_edge_f32 on the widened inputs bit for bit.
+ * In training, out is the forward's rounded 16-bit output, so delta = <grad_out, out> uses the rounded out.  Unknown
+ * dtype: PGLB_EINVAL. */
+int pglb_gat_bwd_edge_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *f, int64_t ldf,
+                          const void *grad_out, int64_t ldg, const void *out, int64_t ldo, const float *attn_src,
+                          const float *attn_dst, const float *lse, float negative_slope, int64_t num_edges, int64_t H,
+                          int64_t head_dim, int dtype, float *alpha_e, float *dz_e, void *stream);
 
 /* out[M, N] = act(x[M, K] @ w[K, N] + bias[N]) -- the dense transform of the conv layers
  * (pgl/nn/conv.py:238-251 GCNConv: `self.linear(...)`, `+ self.bias`, activation; the same Linear in

@@ -13,7 +13,7 @@ PGLB_CUDA_ERR_BASE = 1000
 REDUCE = {"sum": 0, "mean": 1, "max": 2, "min": 3}
 MSG = {"copy": 0, "add": 1, "sub": 2, "mul": 3, "div": 4}
 BCAST_FULL, BCAST_HEAD, BCAST_SCALAR = 0, 1, 2
-DTYPE_BF16, DTYPE_F16 = 1, 2   # dtype of pglb_spmm_csr_x16
+DTYPE_BF16, DTYPE_F16 = 1, 2   # dtype of the *_x16 entries
 
 
 class PglbError(RuntimeError):
@@ -53,6 +53,8 @@ _SIGS = {
                                              _p]),
     "pglb_spmm_csr_x16": (c_int, [_p, _p, _p, _i64, _p, _i64, _i64, _i64, _i64, _i64, c_int, c_int, _p, _p, _p, _p,
                                   _i64, c_int, _p, c_size_t, _p]),
+    "pglb_spmm_csr_ue_x16": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, c_int, _p, _i64, _i64, _i64, _i64, _i64, _i64,
+                                     c_int, c_int, c_int, _p, _p, _i64, c_int, _p, c_size_t, _p]),
     "pglb_narrow_plan_ws": (c_int, [_i64, POINTER(c_size_t)]),
     "pglb_narrow_plan": (c_int, [_p, _p, _p, _i64, _i64, _i64, _p, _p, _p, _p, c_size_t, _p]),
     "pglb_spmm_narrow_ws": (c_int, [_i64, _i64, POINTER(c_size_t)]),
@@ -84,6 +86,13 @@ _SIGS = {
                                              _i64, _i64, _i64, _p, c_size_t, _p]),
     "pglb_gat_bwd_edge_f32": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _p, _p, ctypes.c_float,
                                       _i64, _i64, _i64, _p, _p, _p]),
+    "pglb_gat_fused_csr_x16": (c_int, [_p, _p, _p, _i64, _p, _p, ctypes.c_float, _p, _i64, _i64, _i64, _i64,
+                                       _i64, _i64, c_int, _p, c_size_t, _p]),
+    "pglb_gat_fused_train_csr_x16": (c_int, [_p, _p, _p, _i64, _p, _p, ctypes.c_float, _p, _i64, _p, _i64, _i64,
+                                             _i64, _i64, _i64, c_int, _p, c_size_t, _p]),
+    "pglb_gat_bwd_edge_x16": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _p, _p, ctypes.c_float,
+                                      _i64, _i64, _i64, c_int, _p, _p, _p]),
+    "pglb_head_dots_x16": (c_int, [_p, _i64, _i64, _i64, _i64, c_int, _p, _p, _p, _p, _p]),
     "pglb_gat_attention_csr_f32": (c_int, [_p, _p, _p, _p, ctypes.c_float, _p, _i64, _i64, _i64, _p,
                                            c_size_t, _p]),
     "pglb_sddmm_dot_f32": (c_int, [_p, _p, _p, _i64, _p, _i64, _i64, _i64, _i64, _p, _p]),

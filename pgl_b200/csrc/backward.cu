@@ -109,11 +109,13 @@ __global__ void __launch_bounds__(256) maxmin_bwd_kernel(const int64_t *__restri
 // the forward.  Walks the dst-CSR slots (rows[] = destination of every slot, so G / out / ad / lse are re-read only when
 // the row changes); a warp owns 32 consecutive slots, the D/4 active lanes hold one float4 of the row each, LPH = Dh/4
 // lanes form a head; four gathered feature rows are in flight per lane before the first dot product.
-template <int LPH>
+// T: element type of f, g and out (float, or the 16-bit type of pglb_gat_bwd_edge_x16: a lane reads 8 bytes and widens
+// them exactly, and the arithmetic after that is the float32 kernel's).  a_s, a_d, lse, alpha_e and dz_e are fp32.
+template <int LPH, typename T>
 __global__ void __launch_bounds__(256) gat_bwd_edge_kernel(
     const int64_t *__restrict__ rows, const int64_t *__restrict__ cols, const int64_t *__restrict__ eid,
-    const float *__restrict__ f, int64_t ldf, const float *__restrict__ g, int64_t ldg,
-    const float *__restrict__ out, int64_t ldo, const float *__restrict__ a_s, const float *__restrict__ a_d,
+    const T *__restrict__ f, int64_t ldf, const T *__restrict__ g, int64_t ldg,
+    const T *__restrict__ out, int64_t ldo, const float *__restrict__ a_s, const float *__restrict__ a_d,
     const float *__restrict__ lse, float slope, int64_t E, int H, int D, float *__restrict__ alpha_e,
     float *__restrict__ dz_e) {
     const int lane = threadIdx.x & 31;
@@ -153,7 +155,7 @@ __global__ void __launch_bounds__(256) gat_bwd_edge_kernel(
                 fv[u] = make_float4(0.f, 0.f, 0.f, 0.f);
                 as[u] = 0.f;
                 if (k0 + u < cnt && act) {
-                    fv[u] = __ldg(reinterpret_cast<const float4 *>(f + cc * ldf + lane * 4));
+                    fv[u] = ldg_row4<T>(f + cc * ldf + lane * 4);
                     as[u] = __ldg(a_s + cc * H + head);
                 }
             }
@@ -164,8 +166,8 @@ __global__ void __launch_bounds__(256) gat_bwd_edge_kernel(
                     cur = rr[u];
                     float d = 0.f;
                     if (act) {
-                        g4 = __ldg(reinterpret_cast<const float4 *>(g + cur * ldg + lane * 4));
-                        const float4 o4 = __ldg(reinterpret_cast<const float4 *>(out + cur * ldo + lane * 4));
+                        g4 = ldg_row4<T>(g + cur * ldg + lane * 4);
+                        const float4 o4 = ldg_row4<T>(out + cur * ldo + lane * 4);
                         ad = __ldg(a_d + cur * H + head);
                         ls = __ldg(lse + cur * H + head);
                         d = dot4(g4, o4);
@@ -238,29 +240,35 @@ extern "C" int pglb_edge_softmax_bwd_csr_f32(const int64_t *indptr, const int64_
     return PGLB_OK;
 }
 
-extern "C" int pglb_gat_bwd_edge_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *f,
-                                     int64_t ldf, const float *grad_out, int64_t ldg, const float *out, int64_t ldo,
-                                     const float *attn_src, const float *attn_dst, const float *lse,
-                                     float negative_slope, int64_t num_edges, int64_t H, int64_t head_dim,
-                                     float *alpha_e, float *dz_e, void *stream_) {
+// The checks and the launch of both edge-backward entries.  T: element type of f, grad_out and out; their rows are
+// 16-byte aligned (ld * sizeof(T) % 16 == 0) for either type.
+template <typename T>
+static int gat_bwd_edge_entry(const char *name, const int64_t *rows, const int64_t *cols, const int64_t *eid,
+                              const void *f_, int64_t ldf, const void *grad_out_, int64_t ldg, const void *out_,
+                              int64_t ldo, const float *attn_src, const float *attn_dst, const float *lse,
+                              float negative_slope, int64_t num_edges, int64_t H, int64_t head_dim, float *alpha_e,
+                              float *dz_e, void *stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    PGLB_CHECK_ARG(num_edges >= 0 && H > 0 && head_dim > 0, PGLB_EINVAL, "pglb_gat_bwd_edge_f32: bad size");
+    const T *f = reinterpret_cast<const T *>(f_), *grad_out = reinterpret_cast<const T *>(grad_out_),
+            *out = reinterpret_cast<const T *>(out_);
+    constexpr int64_t B = sizeof(T);
+    PGLB_CHECK_ARG(num_edges >= 0 && H > 0 && head_dim > 0, PGLB_EINVAL, "%s: bad size", name);
     const int64_t D = H * head_dim;
     const int64_t lph = head_dim / 4;
     PGLB_CHECK_ARG(D <= 128 && head_dim % 4 == 0 && (lph & (lph - 1)) == 0, PGLB_EUNSUPPORTED,
-                   "pglb_gat_bwd_edge_f32: needs H*head_dim <= 128 and head_dim in {4, 8, 16, 32, 64, 128}");
+                   "%s: needs H*head_dim <= 128 and head_dim in {4, 8, 16, 32, 64, 128}", name);
     if (num_edges == 0) return PGLB_OK;
     PGLB_CHECK_ARG(rows && cols && f && grad_out && out && attn_src && attn_dst && lse && alpha_e && dz_e, PGLB_EINVAL,
-                   "pglb_gat_bwd_edge_f32: NULL pointer");
+                   "%s: NULL pointer", name);
     auto a16 = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    PGLB_CHECK_ARG(ldf >= D && ldg >= D && ldo >= D && ldf % 4 == 0 && ldg % 4 == 0 && ldo % 4 == 0 && a16(f) &&
-                       a16(grad_out) && a16(out),
-                   PGLB_ESHAPE, "pglb_gat_bwd_edge_f32: rows must be 16-byte aligned");
+    PGLB_CHECK_ARG(ldf >= D && ldg >= D && ldo >= D && (ldf * B) % 16 == 0 && (ldg * B) % 16 == 0 &&
+                       (ldo * B) % 16 == 0 && a16(f) && a16(grad_out) && a16(out),
+                   PGLB_ESHAPE, "%s: rows must be 16-byte aligned", name);
     const int grid = grid_of(num_edges * 1, 64);  // a warp per 32 slots, grid-stride
 #define PGLB_GBE(L)                                                                                                   \
-    gat_bwd_edge_kernel<L><<<grid, 256, 0, stream>>>(rows, cols, eid, f, ldf, grad_out, ldg, out, ldo, attn_src,      \
-                                                    attn_dst, lse, negative_slope, num_edges, (int)H, (int)D,        \
-                                                    alpha_e, dz_e)
+    gat_bwd_edge_kernel<L, T><<<grid, 256, 0, stream>>>(rows, cols, eid, f, ldf, grad_out, ldg, out, ldo, attn_src,   \
+                                                       attn_dst, lse, negative_slope, num_edges, (int)H, (int)D,     \
+                                                       alpha_e, dz_e)
     switch ((int)lph) {
         case 1: PGLB_GBE(1); break;
         case 2: PGLB_GBE(2); break;
@@ -272,6 +280,32 @@ extern "C" int pglb_gat_bwd_edge_f32(const int64_t *rows, const int64_t *cols, c
 #undef PGLB_GBE
     PGLB_LAUNCH_CHECK("gat_bwd_edge_kernel");
     return PGLB_OK;
+}
+
+extern "C" int pglb_gat_bwd_edge_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *f,
+                                     int64_t ldf, const float *grad_out, int64_t ldg, const float *out, int64_t ldo,
+                                     const float *attn_src, const float *attn_dst, const float *lse,
+                                     float negative_slope, int64_t num_edges, int64_t H, int64_t head_dim,
+                                     float *alpha_e, float *dz_e, void *stream_) {
+    return gat_bwd_edge_entry<float>("pglb_gat_bwd_edge_f32", rows, cols, eid, f, ldf, grad_out, ldg, out, ldo,
+                                     attn_src, attn_dst, lse, negative_slope, num_edges, H, head_dim, alpha_e, dz_e,
+                                     stream_);
+}
+
+extern "C" int pglb_gat_bwd_edge_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *f,
+                                     int64_t ldf, const void *grad_out, int64_t ldg, const void *out, int64_t ldo,
+                                     const float *attn_src, const float *attn_dst, const float *lse,
+                                     float negative_slope, int64_t num_edges, int64_t H, int64_t head_dim, int dtype,
+                                     float *alpha_e, float *dz_e, void *stream_) {
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL,
+                   "pglb_gat_bwd_edge_x16: unknown dtype %d", dtype);
+    if (dtype == PGLB_DTYPE_BF16)
+        return gat_bwd_edge_entry<__nv_bfloat16>("pglb_gat_bwd_edge_x16", rows, cols, eid, f, ldf, grad_out, ldg, out,
+                                                 ldo, attn_src, attn_dst, lse, negative_slope, num_edges, H, head_dim,
+                                                 alpha_e, dz_e, stream_);
+    return gat_bwd_edge_entry<__half>("pglb_gat_bwd_edge_x16", rows, cols, eid, f, ldf, grad_out, ldg, out, ldo,
+                                      attn_src, attn_dst, lse, negative_slope, num_edges, H, head_dim, alpha_e, dz_e,
+                                      stream_);
 }
 
 extern "C" int pglb_maxmin_bwd_f32(const int64_t *src_indptr, const int64_t *dst_of_slot,

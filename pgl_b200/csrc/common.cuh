@@ -108,5 +108,12 @@ __device__ __forceinline__ uint2 round4(float4 v) {
     return make_uint2((unsigned)X16<T>::round(v.x) | ((unsigned)X16<T>::round(v.y) << 16),
                       (unsigned)X16<T>::round(v.z) | ((unsigned)X16<T>::round(v.w) << 16));
 }
+// four consecutive elements of a row in global memory (read-only path) as fp32: 16 bytes of float32, or 8 bytes of a
+// 16-bit type widened exactly
+template <typename T>
+__device__ __forceinline__ float4 ldg_row4(const T *p) {
+    if constexpr (sizeof(T) == 4) return __ldg(reinterpret_cast<const float4 *>(p));
+    else return widen4<T>(__ldg(reinterpret_cast<const uint2 *>(p)));
+}
 
 }  // namespace pglb

@@ -288,8 +288,10 @@ __global__ void __launch_bounds__(256) degree_norm_kernel(const int64_t *__restr
 // attn_src = sum(feature * weight_src, -1), attn_dst = sum(feature * weight_dst, -1) -- four elementwise / reduce
 // launches and two [N, H, Dh] temporaries there):  as[n,h] = <f[n,h,:], ws[h,:]>,  ad[n,h] = <f[n,h,:], wd[h,:]>.
 // A warp per row, a float4 per lane, LPH = Dh / 4 lanes per head (shuffle reduce), weights in registers.
-template <int LPH>
-__global__ void __launch_bounds__(256) head_dots_kernel(const float *__restrict__ f, int64_t ldf, int64_t n, int D,
+// T: element type of f (float, or the 16-bit type of pglb_head_dots_x16: 8 bytes per lane, widened exactly, then the
+// float32 kernel's products and adds).  Weights and outputs are fp32.
+template <int LPH, typename T>
+__global__ void __launch_bounds__(256) head_dots_kernel(const T *__restrict__ f, int64_t ldf, int64_t n, int D,
                                                         int H, const float *__restrict__ ws,
                                                         const float *__restrict__ wd, float *__restrict__ as,
                                                         float *__restrict__ ad) {
@@ -315,7 +317,7 @@ __global__ void __launch_bounds__(256) head_dots_kernel(const float *__restrict_
 #pragma unroll
         for (int u = 0; u < U; ++u) {
             v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (act && r0 + u < n) v[u] = __ldg(reinterpret_cast<const float4 *>(f + (r0 + u) * ldf + lane * 4));
+            if (act && r0 + u < n) v[u] = ldg_row4<T>(f + (r0 + u) * ldf + lane * 4);
         }
 #pragma unroll
         for (int u = 0; u < U; ++u) {
@@ -511,20 +513,22 @@ extern "C" int pglb_degree_norm_f32(const int64_t *degree, int64_t n, float *nor
     return PGLB_OK;
 }
 
-extern "C" int pglb_head_dots_f32(const float *f, int64_t ldf, int64_t n, int64_t H, int64_t head_dim,
-                                  const float *w_src, const float *w_dst, float *attn_src, float *attn_dst,
-                                  void *stream_) {
+// The checks and the launch of both head-dots entries.  T: element type of f; rows 16-byte aligned for either type.
+template <typename T>
+static int head_dots_entry(const char *name, const void *f_, int64_t ldf, int64_t n, int64_t H, int64_t head_dim,
+                           const float *w_src, const float *w_dst, float *attn_src, float *attn_dst, void *stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    PGLB_CHECK_ARG(n >= 0 && H > 0 && head_dim > 0, PGLB_EINVAL, "pglb_head_dots_f32: bad size");
+    const T *f = reinterpret_cast<const T *>(f_);
+    PGLB_CHECK_ARG(n >= 0 && H > 0 && head_dim > 0, PGLB_EINVAL, "%s: bad size", name);
     const int64_t D = H * head_dim, lph = head_dim / 4;
     PGLB_CHECK_ARG(D <= 128 && head_dim % 4 == 0 && (lph & (lph - 1)) == 0, PGLB_EUNSUPPORTED,
-                   "pglb_head_dots_f32: needs H*head_dim <= 128 and head_dim in {4, 8, 16, 32, 64, 128}");
+                   "%s: needs H*head_dim <= 128 and head_dim in {4, 8, 16, 32, 64, 128}", name);
     if (n == 0) return PGLB_OK;
-    PGLB_CHECK_ARG(f && w_src && w_dst && attn_src && attn_dst, PGLB_EINVAL, "pglb_head_dots_f32: NULL pointer");
-    PGLB_CHECK_ARG(ldf >= D && ldf % 4 == 0 && a16(f) && a16(w_src) && a16(w_dst), PGLB_ESHAPE,
-                   "pglb_head_dots_f32: rows / weights must be 16-byte aligned");
+    PGLB_CHECK_ARG(f && w_src && w_dst && attn_src && attn_dst, PGLB_EINVAL, "%s: NULL pointer", name);
+    PGLB_CHECK_ARG(ldf >= D && (ldf * (int64_t)sizeof(T)) % 16 == 0 && a16(f) && a16(w_src) && a16(w_dst), PGLB_ESHAPE,
+                   "%s: rows / weights must be 16-byte aligned", name);
     const int grid = grid_for(n * 8);   // a warp per 4 rows
-#define PGLB_HD(L) head_dots_kernel<L><<<grid, 256, 0, stream>>>(f, ldf, n, (int)D, (int)H, w_src, w_dst, attn_src, attn_dst)
+#define PGLB_HD(L) head_dots_kernel<L, T><<<grid, 256, 0, stream>>>(f, ldf, n, (int)D, (int)H, w_src, w_dst, attn_src, attn_dst)
     switch ((int)lph) {
         case 1: PGLB_HD(1); break;
         case 2: PGLB_HD(2); break;
@@ -536,6 +540,25 @@ extern "C" int pglb_head_dots_f32(const float *f, int64_t ldf, int64_t n, int64_
 #undef PGLB_HD
     PGLB_LAUNCH_CHECK("head_dots_kernel");
     return PGLB_OK;
+}
+
+extern "C" int pglb_head_dots_f32(const float *f, int64_t ldf, int64_t n, int64_t H, int64_t head_dim,
+                                  const float *w_src, const float *w_dst, float *attn_src, float *attn_dst,
+                                  void *stream_) {
+    return head_dots_entry<float>("pglb_head_dots_f32", f, ldf, n, H, head_dim, w_src, w_dst, attn_src, attn_dst,
+                                  stream_);
+}
+
+extern "C" int pglb_head_dots_x16(const void *f, int64_t ldf, int64_t n, int64_t H, int64_t head_dim, int dtype,
+                                  const float *w_src, const float *w_dst, float *attn_src, float *attn_dst,
+                                  void *stream_) {
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL,
+                   "pglb_head_dots_x16: unknown dtype %d", dtype);
+    if (dtype == PGLB_DTYPE_BF16)
+        return head_dots_entry<__nv_bfloat16>("pglb_head_dots_x16", f, ldf, n, H, head_dim, w_src, w_dst, attn_src,
+                                              attn_dst, stream_);
+    return head_dots_entry<__half>("pglb_head_dots_x16", f, ldf, n, H, head_dim, w_src, w_dst, attn_src, attn_dst,
+                                   stream_);
 }
 
 // ---- packed column ids + source hotness (L2 residency hint) --------------------------------

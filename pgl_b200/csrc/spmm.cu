@@ -386,7 +386,8 @@ static Shape pick_shape(int64_t D, bool vec4) {
 typedef void (*SpmmKernel)(const SpmmP);
 
 // TI / TO: element types of the kernel's x / out.  A 16-bit type on either side takes the capped kernel at 4 elements
-// per lane and two column iterations; MODE 1 (an edge operand) exists for float32 only.
+// per lane and two column iterations for copy messages.  MODE 1 (an edge operand) exists for float32, and for 16-bit x
+// (pglb_spmm_csr_ue_x16: fp32 y, sum, 4 elements per lane -- the main pass and hub pass 1) with RK 0 only.
 template <typename TI, typename TO, int VEC, int G, int ITERS>
 static SpmmKernel pick_mode(int mode, int rk) {
     if constexpr (sizeof(TI) == 4 && sizeof(TO) == 4) {
@@ -394,11 +395,17 @@ static SpmmKernel pick_mode(int mode, int rk) {
             return rk == 0 ? spmm_csr_kernel<TI, TO, VEC, G, ITERS, 1, 0>
                            : spmm_csr_kernel<TI, TO, VEC, G, ITERS, 1, 1>;
         return rk == 0 ? spmm_csr_kernel<TI, TO, VEC, G, ITERS, 0, 0> : spmm_csr_kernel<TI, TO, VEC, G, ITERS, 0, 1>;
-    } else if constexpr (VEC == 4 && ITERS == 2) {
-        return rk == 0 ? spmm_csr_capped_kernel<TI, TO, VEC, G, ITERS, 0>
-                       : spmm_csr_capped_kernel<TI, TO, VEC, G, ITERS, 1>;
     } else {
-        return rk == 0 ? spmm_csr_kernel<TI, TO, VEC, G, ITERS, 0, 0> : spmm_csr_kernel<TI, TO, VEC, G, ITERS, 0, 1>;
+        if constexpr (sizeof(TI) == 2 && VEC == 4) {
+            if (mode == 1) return spmm_csr_kernel<TI, TO, VEC, G, ITERS, 1, 0>;
+        }
+        if constexpr (VEC == 4 && ITERS == 2) {
+            return rk == 0 ? spmm_csr_capped_kernel<TI, TO, VEC, G, ITERS, 0>
+                           : spmm_csr_capped_kernel<TI, TO, VEC, G, ITERS, 1>;
+        } else {
+            return rk == 0 ? spmm_csr_kernel<TI, TO, VEC, G, ITERS, 0, 0>
+                           : spmm_csr_kernel<TI, TO, VEC, G, ITERS, 0, 1>;
+        }
     }
 }
 
@@ -468,10 +475,15 @@ int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, 
                     const float *y, int64_t ldy, int y_bcast, int head_dim, int msg_op, void *ws,
                     size_t ws_bytes, cudaStream_t stream);
 
-int gat_fused_run(const int64_t *indptr, const int64_t *cols, const float *f, int64_t ldf, float *out,
+// the fused GAT aggregation over f / out of element type T (float, __nv_bfloat16 or __half); gat5_takes: whether its
+// TMA kernel takes a call (16-bit calls must be such calls)
+template <typename T>
+int gat_fused_run(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf, void *out,
                   int64_t ldo, int64_t n_dst, int64_t n_src, int64_t E, int64_t D, int64_t H,
                   const float *attn_src, const float *attn_dst, float slope, float *lse, void *ws, size_t ws_bytes,
                   cudaStream_t stream);
+template <typename T>
+bool gat5_takes(int64_t D, float slope, const void *f, int64_t ldf, const float *attn_src, int64_t H, int64_t n_src);
 
 // spmm_v5_kernel over rows of element type T (float, __nv_bfloat16 or __half): whether it takes a call, and the run
 template <typename T>
@@ -733,28 +745,40 @@ extern "C" int pglb_spmm_csr_x16(const int64_t *indptr, const int64_t *cols, con
     return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
 }
 
-static int gat_fused_entry(const char *name, const int64_t *indptr, const int64_t *cols, const float *f, int64_t ldf,
-                           const float *attn_src, const float *attn_dst, float negative_slope, float *out, int64_t ldo,
+// The argument checks and the launch of the fused GAT entries.  T: element type of f and out.  A 16-bit call also
+// needs 16-byte rows (ldf, ldo % 8 == 0) and a shape the TMA kernel takes; both are checked before any CUDA call.
+template <typename T>
+static int gat_fused_entry(const char *name, const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
+                           const float *attn_src, const float *attn_dst, float negative_slope, void *out, int64_t ldo,
                            float *lse, int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H, int64_t head_dim,
                            void *ws, size_t ws_bytes, void *stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    constexpr int64_t B = sizeof(T);
     PGLB_CHECK_ARG(n_dst >= 0 && n_src >= 0 && num_edges >= 0 && H > 0 && head_dim > 0, PGLB_EINVAL, "%s: bad size", name);
     const int64_t D = H * head_dim;
     PGLB_CHECK_ARG(D <= 128 && head_dim % 4 == 0 && num_edges < 0x7fffffffLL && n_src < 0xffffffffLL,
                    PGLB_EUNSUPPORTED, "%s: needs H*head_dim <= 128 and head_dim %% 4 == 0", name);
     if (n_dst == 0) return PGLB_OK;
     PGLB_CHECK_ARG(indptr && out, PGLB_EINVAL, "%s: NULL pointer", name);
-    PGLB_CHECK_ARG(ldf >= D && ldo >= D && ldf % 4 == 0 && ldo % 4 == 0 && aligned16(f) && aligned16(out),
+    PGLB_CHECK_ARG(ldf >= D && ldo >= D && (ldf * B) % 16 == 0 && (ldo * B) % 16 == 0 && aligned16(f) && aligned16(out),
                    PGLB_ESHAPE, "%s: rows must be 16-byte aligned", name);
+    if constexpr (B == 2) {
+        PGLB_CHECK_ARG(num_edges == 0 || (cols && f && attn_src && attn_dst), PGLB_EINVAL, "%s: NULL pointer", name);
+        PGLB_CHECK_ARG(num_edges == 0 || (ws && (reinterpret_cast<uintptr_t>(ws) & 255u) == 0), PGLB_EWORKSPACE,
+                       "%s: workspace NULL or not 256-byte aligned", name);
+        PGLB_CHECK_ARG(gat5_takes<T>(D, negative_slope, f, ldf, attn_src, H, n_src), PGLB_EUNSUPPORTED,
+                       "%s: shape outside the 16-bit kernel (H %% 4, H <= 32, D %% 8, 16-byte attention rows, "
+                       "0 <= slope <= 1)", name);
+    }
     if (num_edges == 0) {
-        PGLB_CUDA(cudaMemset2DAsync(out, sizeof(float) * ldo, 0, sizeof(float) * D, n_dst, stream));
+        PGLB_CUDA(cudaMemset2DAsync(out, B * ldo, 0, B * D, n_dst, stream));
         return PGLB_OK;
     }
     PGLB_CHECK_ARG(cols && f && attn_src && attn_dst, PGLB_EINVAL, "%s: NULL pointer", name);
     PGLB_CHECK_ARG(ws && (reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
                    "%s: workspace NULL or not 256-byte aligned", name);
-    return gat_fused_run(indptr, cols, f, ldf, out, ldo, n_dst, n_src, num_edges, D, H, attn_src,
-                         attn_dst, negative_slope, lse, ws, ws_bytes, stream);
+    return gat_fused_run<T>(indptr, cols, f, ldf, out, ldo, n_dst, n_src, num_edges, D, H, attn_src, attn_dst,
+                            negative_slope, lse, ws, ws_bytes, stream);
 }
 
 extern "C" int pglb_gat_fused_csr_f32(const int64_t *indptr, const int64_t *cols, const float *f,
@@ -762,8 +786,8 @@ extern "C" int pglb_gat_fused_csr_f32(const int64_t *indptr, const int64_t *cols
                                       float negative_slope, float *out, int64_t ldo, int64_t n_dst,
                                       int64_t n_src, int64_t num_edges, int64_t H, int64_t head_dim,
                                       void *ws, size_t ws_bytes, void *stream_) {
-    return gat_fused_entry("pglb_gat_fused_csr_f32", indptr, cols, f, ldf, attn_src, attn_dst, negative_slope, out, ldo,
-                           nullptr, n_dst, n_src, num_edges, H, head_dim, ws, ws_bytes, stream_);
+    return gat_fused_entry<float>("pglb_gat_fused_csr_f32", indptr, cols, f, ldf, attn_src, attn_dst, negative_slope,
+                                  out, ldo, nullptr, n_dst, n_src, num_edges, H, head_dim, ws, ws_bytes, stream_);
 }
 
 // Training forward: the same launch, which additionally leaves lse[d, h] = log sum_j exp(leaky(as[src_j,h] + ad[d,h]))
@@ -775,6 +799,83 @@ extern "C" int pglb_gat_fused_train_csr_f32(const int64_t *indptr, const int64_t
                                             int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H,
                                             int64_t head_dim, void *ws, size_t ws_bytes, void *stream_) {
     PGLB_CHECK_ARG(lse != nullptr || n_dst == 0, PGLB_EINVAL, "pglb_gat_fused_train_csr_f32: NULL lse");
-    return gat_fused_entry("pglb_gat_fused_train_csr_f32", indptr, cols, f, ldf, attn_src, attn_dst, negative_slope, out,
-                           ldo, lse, n_dst, n_src, num_edges, H, head_dim, ws, ws_bytes, stream_);
+    return gat_fused_entry<float>("pglb_gat_fused_train_csr_f32", indptr, cols, f, ldf, attn_src, attn_dst,
+                                  negative_slope, out, ldo, lse, n_dst, n_src, num_edges, H, head_dim, ws, ws_bytes,
+                                  stream_);
+}
+
+// 16-bit f / out (include/pglb.h): the fp32 entries' arguments plus `dtype`
+extern "C" int pglb_gat_fused_csr_x16(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
+                                      const float *attn_src, const float *attn_dst, float negative_slope, void *out,
+                                      int64_t ldo, int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H,
+                                      int64_t head_dim, int dtype, void *ws, size_t ws_bytes, void *stream_) {
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL,
+                   "pglb_gat_fused_csr_x16: unknown dtype %d", dtype);
+    auto run = [&](auto *elem) -> int {
+        using T = std::remove_pointer_t<decltype(elem)>;
+        return gat_fused_entry<T>("pglb_gat_fused_csr_x16", indptr, cols, f, ldf, attn_src, attn_dst, negative_slope,
+                                  out, ldo, nullptr, n_dst, n_src, num_edges, H, head_dim, ws, ws_bytes, stream_);
+    };
+    return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
+}
+
+extern "C" int pglb_gat_fused_train_csr_x16(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
+                                            const float *attn_src, const float *attn_dst, float negative_slope,
+                                            void *out, int64_t ldo, float *lse, int64_t n_dst, int64_t n_src,
+                                            int64_t num_edges, int64_t H, int64_t head_dim, int dtype, void *ws,
+                                            size_t ws_bytes, void *stream_) {
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL,
+                   "pglb_gat_fused_train_csr_x16: unknown dtype %d", dtype);
+    PGLB_CHECK_ARG(lse != nullptr || n_dst == 0, PGLB_EINVAL, "pglb_gat_fused_train_csr_x16: NULL lse");
+    auto run = [&](auto *elem) -> int {
+        using T = std::remove_pointer_t<decltype(elem)>;
+        return gat_fused_entry<T>("pglb_gat_fused_train_csr_x16", indptr, cols, f, ldf, attn_src, attn_dst,
+                                  negative_slope, out, ldo, lse, n_dst, n_src, num_edges, H, head_dim, ws, ws_bytes,
+                                  stream_);
+    };
+    return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
+}
+
+// Send/recv with an edge operand over 16-bit x / out (include/pglb.h): the node-parallel kernel with MODE 1 -- the
+// reverse-CSR aggregation of the fused GAT backward (grad f = sum over out-edges of alpha * grad_out[dst]).
+extern "C" int pglb_spmm_csr_ue_x16(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const void *x,
+                                    int64_t ldx, const float *y, int64_t ldy, int y_bcast, void *out, int64_t ldo,
+                                    int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t D, int64_t head_dim,
+                                    int dtype, int msg_op, int reduce_op, const float *scale_src,
+                                    const float *scale_dst, int64_t max_degree_hint, int flags, void *ws,
+                                    size_t ws_bytes, void *stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL,
+                   "pglb_spmm_csr_ue_x16: unknown dtype %d", dtype);
+    PGLB_CHECK_ARG(msg_op >= PGLB_MSG_COPY && msg_op <= PGLB_MSG_DIV, PGLB_EINVAL,
+                   "pglb_spmm_csr_ue_x16: unknown msg_op %d", msg_op);
+    PGLB_CHECK_ARG(y_bcast >= PGLB_BCAST_FULL && y_bcast <= PGLB_BCAST_SCALAR, PGLB_EINVAL,
+                   "pglb_spmm_csr_ue_x16: unknown y_bcast %d", y_bcast);
+    {
+        const int rc = spmm_check_args("pglb_spmm_csr_ue_x16", indptr, x, ldx, out, ldo, n_dst, n_src, num_edges, D,
+                                       reduce_op);
+        if (rc) return rc;
+    }
+    PGLB_CHECK_ARG(msg_op == PGLB_MSG_MUL || msg_op == PGLB_MSG_ADD, PGLB_EUNSUPPORTED,
+                   "pglb_spmm_csr_ue_x16: mul / add messages only");
+    PGLB_CHECK_ARG(reduce_op == PGLB_REDUCE_SUM, PGLB_EUNSUPPORTED, "pglb_spmm_csr_ue_x16: sum only");
+    PGLB_CHECK_ARG(y_bcast != PGLB_BCAST_FULL, PGLB_EUNSUPPORTED,
+                   "pglb_spmm_csr_ue_x16: per-head or scalar edge operands only");
+    PGLB_CHECK_ARG(!(flags & PGLB_SPMM_ACCUMULATE), PGLB_EUNSUPPORTED,
+                   "pglb_spmm_csr_ue_x16: PGLB_SPMM_ACCUMULATE would round the output twice");
+    if (n_dst == 0 || D == 0) return PGLB_OK;
+    PGLB_CHECK_ARG(num_edges == 0 || y, PGLB_EINVAL, "pglb_spmm_csr_ue_x16: y is NULL");
+    PGLB_CHECK_ARG(D % 4 == 0, PGLB_EUNSUPPORTED, "pglb_spmm_csr_ue_x16: D %% 4 == 0 needed");
+    if (y_bcast == PGLB_BCAST_HEAD)
+        PGLB_CHECK_ARG(head_dim > 0 && D % head_dim == 0, PGLB_ESHAPE, "pglb_spmm_csr_ue_x16: head_dim must divide D");
+    auto aligned8 = [](const void *q) { return (reinterpret_cast<uintptr_t>(q) & 7u) == 0; };
+    PGLB_CHECK_ARG(ldx % 4 == 0 && ldo % 4 == 0 && aligned8(x) && aligned8(out), PGLB_ESHAPE,
+                   "pglb_spmm_csr_ue_x16: rows must be 8-byte aligned (ldx, ldo %% 4 == 0)");
+    auto run = [&](auto *elem) -> int {
+        using T = std::remove_pointer_t<decltype(elem)>;
+        return spmm_generic_run<T>(indptr, cols, eid, x, ldx, y, ldy, y_bcast, out, ldo, n_dst, num_edges, D,
+                                   head_dim, msg_op, reduce_op, scale_src, scale_dst, max_degree_hint, 0, true, ws,
+                                   ws_bytes, stream);
+    };
+    return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
 }

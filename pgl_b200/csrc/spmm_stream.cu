@@ -755,7 +755,9 @@ __global__ void __launch_bounds__(256) spmm_stream_fixup_kernel(const StreamP p)
 }
 
 // Fused-GAT fix-up: merge the (acc, m, l) partials of a cut row: M = max m_i,
-// out = sum_i acc_i e^{m_i - M} / sum_i l_i e^{m_i - M}
+// out = sum_i acc_i e^{m_i - M} / sum_i l_i e^{m_i - M}.  The partials are fp32; TO is the element type of out (a
+// 16-bit out is rounded once, on the store).
+template <typename TO>
 __global__ void __launch_bounds__(256) spmm_stream_fixup_gat_kernel(const StreamP p) {
     const int lane = threadIdx.x & 31;
     const int64_t t = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -781,7 +783,10 @@ __global__ void __launch_bounds__(256) spmm_stream_fixup_gat_kernel(const Stream
     for (int64_t u = t + 1; u < u_end; ++u) add(2 * u);
     acc.x = __fdiv_rn(acc.x, L); acc.y = __fdiv_rn(acc.y, L);
     acc.z = __fdiv_rn(acc.z, L); acc.w = __fdiv_rn(acc.w, L);
-    *reinterpret_cast<float4 *>(p.out + r * p.ldo + c) = acc;
+    if constexpr (sizeof(TO) == 4)
+        *reinterpret_cast<float4 *>(p.out + r * p.ldo + c) = acc;
+    else
+        *reinterpret_cast<uint2 *>(reinterpret_cast<TO *>(p.out) + r * p.ldo + c) = round4<TO>(acc);
     if (p.lse && c % p.head_dim == 0) p.lse[r * p.ldy + c / p.head_dim] = M + logf(L);
 }
 
@@ -953,7 +958,7 @@ static int launch_stream128(const StreamP &p, cudaStream_t stream) {
     PGLB_LAUNCH_CHECK("spmm_stream128_kernel");
     const int64_t fblocks = (p.ntasks * 32 + 255) / 256;
     if (YM == 2) {
-        spmm_stream_fixup_gat_kernel<<<(unsigned)fblocks, 256, 0, stream>>>(p);
+        spmm_stream_fixup_gat_kernel<float><<<(unsigned)fblocks, 256, 0, stream>>>(p);
     } else {
         spmm_stream_fixup_kernel<float, 1, RK><<<(unsigned)fblocks, 256, 0, stream>>>(p);
     }
@@ -1192,15 +1197,27 @@ int narrow2_run(const uint32_t *plan, const int32_t *nz_row, const int32_t *blk_
     return PGLB_OK;
 }
 
-// Single-pass GAT aggregation (inference): out[d,h,:] = sum_j softmax_j(leaky(as[src_j,h] + ad[d,h])) f[src_j,h,:]
-int gat_fused_run(const int64_t *indptr, const int64_t *cols, const float *f, int64_t ldf, float *out,
+// Whether spmm_gat5_kernel<T> takes a call (the entries' argument checks, before any CUDA call)
+template <typename T>
+bool gat5_takes(int64_t D, float slope, const void *f, int64_t ldf, const float *attn_src, int64_t H, int64_t n_src) {
+    return gat5_eligible<T>(D, slope, f, ldf, attn_src, H, n_src);
+}
+
+// Single-pass GAT aggregation (inference): out[d,h,:] = sum_j softmax_j(leaky(as[src_j,h] + ad[d,h])) f[src_j,h,:].
+// T: element type of f and out.  float32 calls outside gat5 take spmm_stream128_kernel<YM = 2>; a 16-bit call must be
+// one gat5 takes.
+template <typename T>
+int gat_fused_run(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf, void *out,
                   int64_t ldo, int64_t n_dst, int64_t n_src, int64_t E, int64_t D, int64_t H,
                   const float *attn_src, const float *attn_dst, float slope, float *lse, void *ws, size_t ws_bytes,
                   cudaStream_t stream) {
     // the row statistics are written by spmm_gat5_kernel and the merge kernel only
-    const bool tma = gat5_eligible(D, slope, f, ldf, attn_src, H, n_src);
+    const bool tma = gat5_eligible<T>(D, slope, f, ldf, attn_src, H, n_src);
     PGLB_CHECK_ARG(!lse || tma, PGLB_EUNSUPPORTED,
                    "pglb_gat_fused_train_csr_f32: shape outside the TMA kernel (H %% 4, 16-byte rows, 0 <= slope <= 1)");
+    PGLB_CHECK_ARG(sizeof(T) == 4 || tma, PGLB_EUNSUPPORTED,
+                   "pglb_gat_fused_csr_x16: shape outside the 16-bit kernel (H %% 4, H <= 32, D %% 8, 16-byte rows, "
+                   "0 <= slope <= 1)");
     StreamP p{};
     p.y = attn_src;
     p.ldy = H;
@@ -1216,12 +1233,20 @@ int gat_fused_run(const int64_t *indptr, const int64_t *cols, const float *f, in
     }
     p.dyn = dyn_mode("PGLB_GAT_DYN", 1, p.ntasks);
     {
-        const int rc = launch_empty_rows<float>(p, stream);
+        const int rc = launch_empty_rows<T>(p, stream);
         if (rc) return rc;
     }
-    if (tma) return launch_gat5(p, attn_src, H, stream);
-    return launch_stream128<0, false, 0, 2>(p, stream);
+    if (tma) return launch_gat5<T>(p, attn_src, H, stream);
+    if constexpr (sizeof(T) == 4) return launch_stream128<0, false, 0, 2>(p, stream);
+    return PGLB_EUNSUPPORTED;   // not reached: refused above
 }
+
+// the instantiations the entries in spmm.cu call
+template decltype(gat5_takes<__nv_bfloat16>) gat5_takes<__nv_bfloat16>;
+template decltype(gat5_takes<__half>) gat5_takes<__half>;
+template decltype(gat_fused_run<float>) gat_fused_run<float>;
+template decltype(gat_fused_run<__nv_bfloat16>) gat_fused_run<__nv_bfloat16>;
+template decltype(gat_fused_run<__half>) gat_fused_run<__half>;
 
 }  // namespace pglb
 

@@ -6,6 +6,7 @@ aggregation in two ``* norm`` multiplies, both ride inside the aggregation kerne
 Parameter layout follows paddle.nn.Linear: ``weight`` is [in, out] and y = x @ weight + bias,
 so reference checkpoints map one to one.
 """
+import functools
 import math as _math
 
 import torch
@@ -155,6 +156,10 @@ class GCNConv(nn.Module):
         return output
 
 
+# feature dtypes of GATConv's fused training path (16-bit: the *_x16 kernels)
+_FUSED_TRAIN_DTYPES = (torch.float32, torch.bfloat16, torch.float16)
+
+
 class GATConv(nn.Module):
     """reference pgl/nn/conv.py:257-346."""
 
@@ -183,12 +188,19 @@ class GATConv(nn.Module):
         feature = self.linear(feature)
         feature = feature.reshape(-1, self.num_heads, self.hidden_size)
         from .. import ops as _ops
+        # the dtype of the attention logits and of the layer's output: torch's promotion of the features' and the
+        # attention weights' dtypes (a bf16 module gives bf16, bf16 features under fp32 weights give fp32)
+        out_dtype = functools.reduce(torch.promote_types, (feature.dtype, self.weight_src.dtype, self.weight_dst.dtype))
         dots = _ops.head_dots(feature, self.weight_src, self.weight_dst) if feature.is_cuda else None
-        if dots is not None:      # both projections in one pass over the features
+        if dots is not None:      # both projections in one pass over the features (float32 logits)
             attn_src, attn_dst = dots
         else:
             attn_src = torch.sum(feature * self.weight_src, dim=-1)
             attn_dst = torch.sum(feature * self.weight_dst, dim=-1)
+
+        def unfused_attn():
+            # the op-by-op paths take the logits in the layer's dtype, as the two torch expressions give them
+            return attn_src.to(out_dtype), attn_dst.to(out_dtype)
         no_attn_drop = self.attn_drop <= 1e-15 or not self.training
         if not torch.is_grad_enabled() and no_attn_drop and type(graph).__name__ == "Graph":
             # inference: send_uv + LeakyReLU + edge_softmax in one kernel (logits never stored),
@@ -197,8 +209,10 @@ class GATConv(nn.Module):
             csr = graph._fwd_csr()
             # one pass when the row fits the wide-row kernel (H*Dh in (64, 128]); otherwise the
             # fused attention kernel + slot-ordered aggregation
-            output = ops.gat_fused(csr, feature, attn_src, attn_dst, self.leaky_relu.negative_slope)
+            output = ops.gat_fused(csr, feature, attn_src, attn_dst, self.leaky_relu.negative_slope,
+                                   out_dtype=out_dtype)
             if output is None:
+                attn_src, attn_dst = unfused_attn()
                 alpha = ops.gat_attention_csr(csr, attn_src, attn_dst, self.leaky_relu.negative_slope)
                 output = ops.aggregate_ue_slots(feature, alpha.reshape(-1, self.num_heads, 1), csr,
                                                 int(feature.shape[0]), "mul", "sum")
@@ -210,13 +224,14 @@ class GATConv(nn.Module):
                 output = self.activation(output)
             return output
         output = None
-        if no_attn_drop and type(graph).__name__ == "Graph" and feature.dtype == torch.float32:
+        if no_attn_drop and type(graph).__name__ == "Graph" and feature.dtype in _FUSED_TRAIN_DTYPES:
             # training without attention dropout: the same single-pass kernel, which keeps the rows' log-sum-exp, and
             # a fused backward (ops._GatFused); None when the shape is outside it
             from .. import ops
             output = ops.gat_fused_train(graph._fwd_csr(), graph._bwd_csr, feature, attn_src, attn_dst,
-                                         self.leaky_relu.negative_slope)
+                                         self.leaky_relu.negative_slope, out_dtype=out_dtype)
         if output is None:
+            attn_src, attn_dst = unfused_attn()
             alpha = graph.send_uv(attn_src, attn_dst, "add")
             alpha = self.leaky_relu(alpha)
             alpha = GF.edge_softmax(graph, alpha)

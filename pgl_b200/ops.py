@@ -290,11 +290,18 @@ def _spmm_raw(indptr, cols, x2, n_dst, reduce_op, eid=None, y2=None, y_bcast=BCA
               head_dim=1, msg_op="copy", scale_src=None, scale_dst=None, max_degree=-1,
               num_edges=None, out=None, packed=None, accumulate=False):
     """float32 x: pglb_spmm_csr_slot_scale_f32, or pglb_spmm_narrow_f32 with a NarrowPlan.  bfloat16 / float16 x:
-    copy messages only, through pglb_spmm_csr_x16.  The output has x's dtype."""
+    copy messages through pglb_spmm_csr_x16; a per-head or scalar float32 edge operand with mul / add messages and sum
+    (the fused GAT backward's grad f) through pglb_spmm_csr_ue_x16.  The output has x's dtype."""
     half = x2.dtype in HALF_DTYPES
-    if half and (msg_op != "copy" or y2 is not None or accumulate):
-        raise TypeError("pgl_b200: 16-bit features aggregate copy messages only (got msg_op=%s%s%s)"
-                        % (msg_op, ", an edge operand" if y2 is not None else "", ", accumulate" if accumulate else ""))
+    half_ue = (half and y2 is not None and msg_op in ("mul", "add") and reduce_op == "sum" and not accumulate
+               and y_bcast in (BCAST_HEAD, BCAST_SCALAR))
+    if half and not half_ue and (msg_op != "copy" or y2 is not None or accumulate):
+        raise TypeError("pgl_b200: 16-bit features aggregate copy messages, or mul / add messages with a per-head or "
+                        "scalar edge operand into a sum (got msg_op=%s, reduce_op=%s%s%s)"
+                        % (msg_op, reduce_op, ", an edge operand" if y2 is not None else "",
+                           ", accumulate" if accumulate else ""))
+    if half_ue and y2.dtype != torch.float32:
+        y2 = y2.float()
     dev = x2.device
     D = int(x2.shape[1])
     E = int(num_edges if num_edges is not None else (cols.shape[0] if cols is not None else 0))
@@ -334,7 +341,13 @@ def _spmm_raw(indptr, cols, x2, n_dst, reduce_op, eid=None, y2=None, y_bcast=BCA
     ids = _ptr(packed[0]) if packed is not None else None
     flags = (1 if accumulate else 0) | (2 if (packed is not None and packed[1]) else 0)
     with torch.cuda.device(dev):
-        if half:
+        if half_ue:
+            check(lib.pglb_spmm_csr_ue_x16(
+                _ptr(indptr), _ptr(cols), _ptr(eid), _ptr(x2), x2.stride(0), _ptr(y2), y2.stride(0), y_bcast,
+                _ptr(out), out.stride(0), n_dst, int(x2.shape[0]), E, D, head_dim, _DTYPE16[x2.dtype], MSG[msg_op],
+                REDUCE[reduce_op], _ptr(scale_src), _ptr(scale_dst), int(max_degree), 0, _ptr(ws), ws.numel(),
+                _stream()))
+        elif half:
             check(lib.pglb_spmm_csr_x16(
                 _ptr(indptr), _ptr(cols), _ptr(x2), x2.stride(0), _ptr(out), out.stride(0), n_dst, int(x2.shape[0]),
                 E, D, _DTYPE16[x2.dtype], REDUCE[reduce_op], _ptr(scale_src), _ptr(sslot), _ptr(scale_dst), ids,
@@ -1156,14 +1169,68 @@ def gat_attention_csr(csr, attn_src, attn_dst, negative_slope=0.2):
     return out
 
 
-@f64_through
-def gat_fused(csr, f, attn_src, attn_dst, negative_slope=0.2):
+def _result_dtype(out_dtype, *tensors):
+    """out_dtype, or torch's promotion of the tensors' dtypes when it is None."""
+    if out_dtype is not None:
+        return out_dtype
+    return functools.reduce(torch.promote_types, [t.dtype for t in tensors])
+
+
+def _att32(a):
+    """Attention logits of the 16-bit GAT routes as a float32 [N, H] tensor (an N x H cast for 16-bit ones)."""
+    mat = getattr(a, "materialize", None)
+    a = mat() if mat is not None else a
+    return _f32_2d(a.float() if a.dtype in HALF_DTYPES else a)
+
+
+def _gat_fused_x16(csr, f, attn_src, attn_dst, negative_slope):
+    """pglb_gat_fused_csr_x16 on 16-bit f; None when the kernel does not take the shape or layout."""
+    n, H, Dh = int(f.shape[0]), int(f.shape[1]), int(f.shape[2])
+    f2 = _f32_2d(f, allow16=True)
+    a_s, a_d = _att32(attn_src), _att32(attn_dst)
+    E = int(csr["cols"].shape[0])
+    n_dst = int(csr["indptr"].shape[0]) - 1
+    out = torch.empty((n_dst, H * Dh), dtype=f2.dtype, device=f2.device)
+    need = ctypes.c_size_t(0)
+    check(lib.pglb_spmm_csr_ws(n_dst, E, H * Dh, ctypes.byref(need)))
+    ws = workspace(f2.device, need.value)
+    try:
+        with torch.cuda.device(f2.device):
+            check(lib.pglb_gat_fused_csr_x16(_ptr(csr["indptr"]), _ptr(csr["cols"]), _ptr(f2), f2.stride(0),
+                                             _ptr(a_s), _ptr(a_d), float(negative_slope), _ptr(out),
+                                             out.stride(0), n_dst, n, E, H, Dh, _DTYPE16[f2.dtype], _ptr(ws),
+                                             ws.numel(), _stream()))
+    except _lib.PglbError as ex:
+        if ex.code in (-2, -4):   # PGLB_ESHAPE / PGLB_EUNSUPPORTED: checked before any device work
+            return None
+        raise
+    return out.reshape(n_dst, H, Dh)
+
+
+def gat_fused(csr, f, attn_src, attn_dst, negative_slope=0.2, out_dtype=None):
     """Single-pass GAT aggregation (online softmax in the wide-row kernel).  f [N, H, Dh] with
-    H*Dh <= 128 and Dh % 4 == 0; returns [N, H, Dh], or None when the shape is not supported."""
+    H*Dh <= 128 and Dh % 4 == 0; returns [N, H, Dh], or None when the shape is not supported.
+    The result has dtype ``out_dtype``, or by default torch's promotion of f's and the attention's dtypes.  When f is
+    bfloat16 / float16 and the result has f's dtype, the 16-bit kernel runs on f as it is (attention widened to
+    float32): the result equals the float32 kernel's on the widened f, rounded once.  Other calls, and 16-bit shapes
+    that kernel does not take, run the float32 kernel on widened inputs and round its result to the result dtype."""
     require_cuda(f, attn_src, attn_dst)
     n, H, Dh = int(f.shape[0]), int(f.shape[1]), int(f.shape[2])
     if H * Dh > 128 or Dh % 4 or H * Dh <= 64:
         return None
+    res = _result_dtype(out_dtype, f, attn_src, attn_dst)
+    if f.dtype in HALF_DTYPES and res == f.dtype and torch.float64 not in (attn_src.dtype, attn_dst.dtype):
+        out = _gat_fused_x16(csr, f, attn_src, attn_dst, negative_slope)
+        if out is not None:
+            return out
+    out = _gat_fused_f32(csr, f, attn_src, attn_dst, negative_slope)
+    return out if out_dtype is None or out.dtype == out_dtype else out.to(out_dtype)
+
+
+@f64_through
+def _gat_fused_f32(csr, f, attn_src, attn_dst, negative_slope=0.2):
+    """gat_fused on the float32 kernel (other float dtypes through f64_through)."""
+    n, H, Dh = int(f.shape[0]), int(f.shape[1]), int(f.shape[2])
     f2 = _f32_2d(f)
     a_s, a_d = _f32_2d(attn_src), _f32_2d(attn_dst)
     E = int(csr["cols"].shape[0])
@@ -1181,8 +1248,9 @@ def gat_fused(csr, f, attn_src, attn_dst, negative_slope=0.2):
 
 
 class _HeadDots(torch.autograd.Function):
-    """attn_src / attn_dst of GATConv in one pass over the features (pglb_head_dots_f32); the backward is three
-    elementwise / reduce torch ops on the gradient path."""
+    """attn_src / attn_dst of GATConv in one pass over the features (pglb_head_dots_f32, or pglb_head_dots_x16 for
+    16-bit f); the backward is three elementwise / reduce torch ops on the gradient path, formed in float32 and
+    returned in each input's dtype."""
 
     @staticmethod
     def forward(ctx, f3, w_src, w_dst):
@@ -1190,10 +1258,14 @@ class _HeadDots(torch.autograd.Function):
         f2 = f3.reshape(n, H * Dh)
         a_s = torch.empty((n, H), dtype=torch.float32, device=f3.device)
         a_d = torch.empty((n, H), dtype=torch.float32, device=f3.device)
-        ws, wd = w_src.contiguous(), w_dst.contiguous()
+        ws, wd = w_src.float().contiguous(), w_dst.float().contiguous()   # an H x Dh cast for 16-bit weights
         with torch.cuda.device(f3.device):
-            check(lib.pglb_head_dots_f32(_ptr(f2), f2.stride(0), n, H, Dh, _ptr(ws), _ptr(wd), _ptr(a_s), _ptr(a_d),
-                                         _stream()))
+            if f3.dtype in HALF_DTYPES:
+                check(lib.pglb_head_dots_x16(_ptr(f2), f2.stride(0), n, H, Dh, _DTYPE16[f3.dtype], _ptr(ws),
+                                             _ptr(wd), _ptr(a_s), _ptr(a_d), _stream()))
+            else:
+                check(lib.pglb_head_dots_f32(_ptr(f2), f2.stride(0), n, H, Dh, _ptr(ws), _ptr(wd), _ptr(a_s),
+                                             _ptr(a_d), _stream()))
         ctx.save_for_backward(f3, w_src, w_dst)
         return a_s, a_d
 
@@ -1202,27 +1274,35 @@ class _HeadDots(torch.autograd.Function):
         f3, w_src, w_dst = ctx.saved_tensors
         gf = gw_s = gw_d = None
         if ctx.needs_input_grad[0]:
-            gf = g_s.unsqueeze(-1) * w_src + g_d.unsqueeze(-1) * w_dst
+            gf = (g_s.unsqueeze(-1) * w_src.float() + g_d.unsqueeze(-1) * w_dst.float()).to(f3.dtype)
         if ctx.needs_input_grad[1]:
-            gw_s = (g_s.unsqueeze(-1) * f3).sum(0).reshape(w_src.shape)
+            gw_s = (g_s.unsqueeze(-1) * f3.float()).sum(0).reshape(w_src.shape).to(w_src.dtype)
         if ctx.needs_input_grad[2]:
-            gw_d = (g_d.unsqueeze(-1) * f3).sum(0).reshape(w_dst.shape)
+            gw_d = (g_d.unsqueeze(-1) * f3.float()).sum(0).reshape(w_dst.shape).to(w_dst.dtype)
         return gf, gw_s, gw_d
 
 
 def head_dots(f, w_src, w_dst):
     """(sum(f * w_src, -1), sum(f * w_dst, -1)) for f [N, H, Dh], w [H, Dh] (or [1, H, Dh]) -- GATConv's attention
     projections, reference pgl/nn/conv.py:323-326 -- or None when the shape is outside the kernel (the caller keeps
-    the two torch expressions)."""
-    if f.dim() != 3 or not f.is_cuda or f.dtype != torch.float32 or w_src.dtype != torch.float32:
+    the two torch expressions).  f float32 with float32 weights, or bfloat16 / float16 f with weights in float32 or
+    f's dtype; the projections are float32 (for 16-bit f: the float32 kernel's result on the widened f and weights)."""
+    if f.dim() != 3 or not f.is_cuda:
+        return None
+    if not (f.dtype == torch.float32 or f.dtype in HALF_DTYPES):
+        return None
+    if any(w.dtype not in (torch.float32, f.dtype) for w in (w_src, w_dst)):
         return None
     n, H, Dh = (int(v) for v in f.shape)
     lph = Dh // 4
     if H * Dh > 128 or Dh % 4 or (lph & (lph - 1)) or w_src.numel() != H * Dh or w_dst.numel() != H * Dh:
         return None
+    if (H * Dh * f.element_size()) % 16:
+        return None     # the kernel reads 16-byte rows: a 16-bit row needs H*Dh % 8 == 0 (e.g. not 3 heads x 4)
     if not f.is_contiguous():
         f = f.contiguous()
-    if f.data_ptr() % 16 or w_src.data_ptr() % 16 or w_dst.data_ptr() % 16:
+    # float32 weights reach the kernel as they are (16-bit ones are widened into a fresh, aligned copy)
+    if f.data_ptr() % 16 or any(w.dtype == torch.float32 and w.data_ptr() % 16 for w in (w_src, w_dst)):
         return None
     return _HeadDots.apply(f, w_src, w_dst)
 
@@ -1231,22 +1311,29 @@ class _GatFused(torch.autograd.Function):
     """The single-pass GAT aggregation under autograd (reference pgl/nn/conv.py:333-339 differentiated by Paddle over
     four ops).  Forward = pglb_gat_fused_train_csr_f32 (one launch; keeps only lse[N, H]).  Backward = one edge kernel
     (pglb_gat_bwd_edge_f32: alpha rebuilt, SDDMM dot, softmax and LeakyReLU backward) + three reverse-CSR aggregations
-    on the existing kernels."""
+    on the existing kernels.  16-bit f2: the *_x16 entries; out and grad f in f2's dtype, lse, alpha, dz and the
+    attention and its gradients float32 (a_s / a_d are float32 here)."""
 
     @staticmethod
     def forward(ctx, f2, a_s, a_d, fwd, bwd, slope, H, Dh):
         n = int(f2.shape[0])
         E = int(fwd["cols"].shape[0])
         n_dst = int(fwd["indptr"].shape[0]) - 1
-        out = torch.empty((n_dst, H * Dh), dtype=torch.float32, device=f2.device)
+        out = torch.empty((n_dst, H * Dh), dtype=f2.dtype, device=f2.device)
         lse = torch.zeros((n_dst, H), dtype=torch.float32, device=f2.device)
         need = ctypes.c_size_t(0)
         check(lib.pglb_spmm_csr_ws(n_dst, E, H * Dh, ctypes.byref(need)))
         ws = workspace(f2.device, need.value)
         with torch.cuda.device(f2.device):
-            check(lib.pglb_gat_fused_train_csr_f32(_ptr(fwd["indptr"]), _ptr(fwd["cols"]), _ptr(f2), f2.stride(0),
-                                                   _ptr(a_s), _ptr(a_d), float(slope), _ptr(out), out.stride(0),
-                                                   _ptr(lse), n_dst, n, E, H, Dh, _ptr(ws), ws.numel(), _stream()))
+            if f2.dtype in HALF_DTYPES:
+                check(lib.pglb_gat_fused_train_csr_x16(
+                    _ptr(fwd["indptr"]), _ptr(fwd["cols"]), _ptr(f2), f2.stride(0), _ptr(a_s), _ptr(a_d), float(slope),
+                    _ptr(out), out.stride(0), _ptr(lse), n_dst, n, E, H, Dh, _DTYPE16[f2.dtype], _ptr(ws), ws.numel(),
+                    _stream()))
+            else:
+                check(lib.pglb_gat_fused_train_csr_f32(
+                    _ptr(fwd["indptr"]), _ptr(fwd["cols"]), _ptr(f2), f2.stride(0), _ptr(a_s), _ptr(a_d), float(slope),
+                    _ptr(out), out.stride(0), _ptr(lse), n_dst, n, E, H, Dh, _ptr(ws), ws.numel(), _stream()))
         ctx.meta = (fwd, bwd, float(slope), H, Dh)
         ctx.save_for_backward(f2, a_s, a_d, out, lse)
         return out
@@ -1256,15 +1343,23 @@ class _GatFused(torch.autograd.Function):
         fwd, bwd, slope, H, Dh = ctx.meta
         bwd = bwd() if callable(bwd) else bwd
         f2, a_s, a_d, out, lse = ctx.saved_tensors
-        g = _f32_2d(g)
+        half = f2.dtype in HALF_DTYPES
+        g = _f32_2d(g.to(f2.dtype) if g.dtype != f2.dtype else g, allow16=half)
         E = int(fwd["cols"].shape[0])
         n_src, n_dst = int(f2.shape[0]), int(out.shape[0])
         alpha = torch.empty((E, H), dtype=torch.float32, device=g.device)
         dz = torch.empty((E, H), dtype=torch.float32, device=g.device)
         with torch.cuda.device(g.device):
-            check(lib.pglb_gat_bwd_edge_f32(_ptr(fwd["rows"]), _ptr(fwd["cols"]), _ptr(fwd["eid"]), _ptr(f2),
-                                            f2.stride(0), _ptr(g), g.stride(0), _ptr(out), out.stride(0), _ptr(a_s),
-                                            _ptr(a_d), _ptr(lse), slope, E, H, Dh, _ptr(alpha), _ptr(dz), _stream()))
+            if half:
+                check(lib.pglb_gat_bwd_edge_x16(_ptr(fwd["rows"]), _ptr(fwd["cols"]), _ptr(fwd["eid"]), _ptr(f2),
+                                                f2.stride(0), _ptr(g), g.stride(0), _ptr(out), out.stride(0),
+                                                _ptr(a_s), _ptr(a_d), _ptr(lse), slope, E, H, Dh, _DTYPE16[f2.dtype],
+                                                _ptr(alpha), _ptr(dz), _stream()))
+            else:
+                check(lib.pglb_gat_bwd_edge_f32(_ptr(fwd["rows"]), _ptr(fwd["cols"]), _ptr(fwd["eid"]), _ptr(f2),
+                                                f2.stride(0), _ptr(g), g.stride(0), _ptr(out), out.stride(0),
+                                                _ptr(a_s), _ptr(a_d), _ptr(lse), slope, E, H, Dh, _ptr(alpha),
+                                                _ptr(dz), _stream()))
         gf = gs = gd = None
         if ctx.needs_input_grad[0]:   # grad f[s] = sum over the out-edges of s of alpha[e] * g[dst[e]]
             gf = _spmm_raw(bwd["indptr"], bwd["cols"], g, n_src, "sum", eid=bwd["eid"], y2=alpha, y_bcast=BCAST_HEAD,
@@ -1279,22 +1374,31 @@ class _GatFused(torch.autograd.Function):
 GAT_FUSED_TRAIN = os.environ.get("PGLB_GAT_FUSED_TRAIN", "1") != "0"
 
 
-def gat_fused_train(fwd, bwd, f, attn_src, attn_dst, negative_slope=0.2):
-    """gat_fused with a backward (float32 only).  f [N, H, Dh], 64 < H*Dh <= 128, H % 4 == 0, Dh a power of two >= 4,
+def gat_fused_train(fwd, bwd, f, attn_src, attn_dst, negative_slope=0.2, out_dtype=None):
+    """gat_fused with a backward.  f [N, H, Dh], 64 < H*Dh <= 128, H % 4 == 0, Dh a power of two >= 4,
     0 <= slope <= 1; returns [N, H, Dh], or None when the shape is outside the fused kernels (the caller keeps the
-    op-by-op path).  ``bwd`` is the reverse CSR dict or a callable returning it."""
+    op-by-op path).  ``bwd`` is the reverse CSR dict or a callable returning it.
+    The result dtype is ``out_dtype``, or by default torch's promotion of f's and the attention's dtypes.  float32 f
+    runs the float32 kernels (the result cast to the result dtype).  bfloat16 / float16 f runs the 16-bit kernels when
+    the result dtype is f's (attention widened to float32; grad f in f's dtype, grad attention formed in float32 and
+    returned in the attention's dtype); other 16-bit calls return None."""
     require_cuda(f, attn_src, attn_dst)
     n, H, Dh = int(f.shape[0]), int(f.shape[1]), int(f.shape[2])
-    if not GAT_FUSED_TRAIN or f.dtype != torch.float32 or H * Dh > 128 or H * Dh <= 64 or H % 4 or H > 32:
+    half = f.dtype in HALF_DTYPES
+    res = _result_dtype(out_dtype, f, attn_src, attn_dst)
+    if not GAT_FUSED_TRAIN or H * Dh > 128 or H * Dh <= 64 or H % 4 or H > 32:
+        return None
+    if not (f.dtype == torch.float32 or (half and res == f.dtype and torch.float64 not in (attn_src.dtype,
+                                                                                          attn_dst.dtype))):
         return None
     if Dh < 4 or (Dh & (Dh - 1)) or not (0.0 <= float(negative_slope) <= 1.0):
         return None
     n_dst = int(fwd["indptr"].shape[0]) - 1
     if n_dst != n or int(fwd["cols"].shape[0]) == 0 or fwd.get("rows") is None:
         return None
-    f2 = _f32_2d(f)
-    a_s, a_d = _f32_2d(attn_src), _f32_2d(attn_dst)
-    if f2.data_ptr() % 16 or (f2.stride(0) * 4) % 16 or a_s.data_ptr() % 16:
+    f2 = _f32_2d(f, allow16=half)
+    a_s, a_d = (_att32(attn_src), _att32(attn_dst)) if half else (_f32_2d(attn_src), _f32_2d(attn_dst))
+    if f2.data_ptr() % 16 or (f2.stride(0) * f2.element_size()) % 16 or a_s.data_ptr() % 16:
         return None
     try:
         out = _GatFused.apply(f2, a_s, a_d, fwd, bwd, float(negative_slope), H, Dh)
@@ -1302,7 +1406,8 @@ def gat_fused_train(fwd, bwd, f, attn_src, attn_dst, negative_slope=0.2):
         if ex.code == -4:   # PGLB_EUNSUPPORTED: e.g. 32 heads, whose attention rows do not fit the kernel's rings
             return None
         raise
-    return out.reshape(n_dst, H, Dh)
+    out = out.reshape(n_dst, H, Dh)
+    return out if out.dtype == res else out.to(res)
 
 
 @f64_through
