@@ -354,6 +354,49 @@ int pglb_gat_bwd_edge_x16(const int64_t *rows, const int64_t *cols, const int64_
                           const float *attn_dst, const float *lse, float negative_slope, int64_t num_edges, int64_t H,
                           int64_t head_dim, int dtype, float *alpha_e, float *dz_e, void *stream);
 
+/* Training with attention dropout (pgl/nn/conv.py:337-339: dropout on the normalised attention, per edge and head):
+ *   out[d,h,:] = sum_j s * m[j,h] * alpha[j,h] * f[cols[j],h,:],   m in {0, 1},  s = (float)(1 / (1 - attn_drop)).
+ *   - The stream: the keep bit m of dst-CSR slot j (absolute slot index) and head h is word h % 4 of
+ *     Philox4x32-10(counter = (j lo32, j hi32, h / 4, (uint32_t)(offset / 4)), key = (seed lo32, seed hi32)), kept iff
+ *     word >= thresh = min(floor(attn_drop * 2^32), 2^32 - 1).  thresh and s are derived in double from the float
+ *     attn_drop.  The forward and the backward recompute m in registers from (seed, offset); no mask is stored.
+ *     pglb_attn_dropout_keep_host gives the same bits on the host.
+ *   - Forward (pglb_gat_fused_train_drop_csr_*): the train entries' arguments plus attn_drop, seed, offset.  The
+ *     online softmax's running sum keeps every slot and only the accumulator skips dropped ones, so lse is bitwise
+ *     the train entry's lse; the row's quotient is multiplied by s once, after the division.
+ *   - Backward (pglb_gat_bwd_edge_drop_*): the edge entries' arguments plus the forward's attn_drop, seed, offset.
+ *     d alpha = s m <grad_out, f[src]>; delta = <grad_out, out> is unchanged; alpha_e holds the dropped attention
+ *     beta = m ? fl(alpha * s) : 0, with which grad f is aggregated as before.
+ *   - Bit anchors: attn_drop = 1e-12 (thresh 0, s = 1.0f) keeps every slot and gives out, lse, alpha_e and dz_e
+ *     bitwise equal to the entries without dropout; the *_x16 siblings relate to the f32 ones as without dropout.
+ *   - attn_drop outside (0, 1) (NaN included) or offset % 4 != 0: PGLB_EINVAL, checked before anything else and before
+ *     any CUDA call.  H % 4 != 0 and the shapes the siblings refuse: PGLB_EUNSUPPORTED. */
+int pglb_gat_fused_train_drop_csr_f32(const int64_t *indptr, const int64_t *cols, const float *f, int64_t ldf,
+                                      const float *attn_src, const float *attn_dst, float negative_slope, float *out,
+                                      int64_t ldo, float *lse, int64_t n_dst, int64_t n_src, int64_t num_edges,
+                                      int64_t H, int64_t head_dim, float attn_drop, uint64_t seed, uint64_t offset,
+                                      void *ws, size_t ws_bytes, void *stream);
+int pglb_gat_fused_train_drop_csr_x16(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
+                                      const float *attn_src, const float *attn_dst, float negative_slope, void *out,
+                                      int64_t ldo, float *lse, int64_t n_dst, int64_t n_src, int64_t num_edges,
+                                      int64_t H, int64_t head_dim, int dtype, float attn_drop, uint64_t seed,
+                                      uint64_t offset, void *ws, size_t ws_bytes, void *stream);
+int pglb_gat_bwd_edge_drop_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *f,
+                               int64_t ldf, const float *grad_out, int64_t ldg, const float *out, int64_t ldo,
+                               const float *attn_src, const float *attn_dst, const float *lse, float negative_slope,
+                               int64_t num_edges, int64_t H, int64_t head_dim, float attn_drop, uint64_t seed,
+                               uint64_t offset, float *alpha_e, float *dz_e, void *stream);
+int pglb_gat_bwd_edge_drop_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *f,
+                               int64_t ldf, const void *grad_out, int64_t ldg, const void *out, int64_t ldo,
+                               const float *attn_src, const float *attn_dst, const float *lse, float negative_slope,
+                               int64_t num_edges, int64_t H, int64_t head_dim, int dtype, float attn_drop,
+                               uint64_t seed, uint64_t offset, float *alpha_e, float *dz_e, void *stream);
+/* keep_words[i] = the keep word of dst-CSR slot slot0 + i (bit h = head h kept) of the stream above, computed on the
+ * host by the kernels' own function.  H % 4 == 0, 4 <= H <= 32 (else PGLB_EUNSUPPORTED); attn_drop and offset as
+ * above; n_slots = 0 does nothing. */
+int pglb_attn_dropout_keep_host(uint64_t seed, uint64_t offset, float attn_drop, int64_t slot0, int64_t n_slots,
+                                int64_t H, uint32_t *keep_words);
+
 /* out[M, N] = act(x[M, K] @ w[K, N] + bias[N]) -- the dense transform of the conv layers
  * (pgl/nn/conv.py:238-251 GCNConv: `self.linear(...)`, `+ self.bias`, activation; the same Linear in
  * GATConv :321 / GraphSageConv :107-108) on the tensor cores with 3xTF32 error compensation (fp32-level

@@ -34,6 +34,7 @@ lib = _load()
 
 _p = c_void_p
 _i64 = c_int64
+_u64 = ctypes.c_uint64
 
 _SIGS = {
     "pglb_version": (c_int, []),
@@ -93,6 +94,16 @@ _SIGS = {
     "pglb_gat_bwd_edge_x16": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _p, _p, ctypes.c_float,
                                       _i64, _i64, _i64, c_int, _p, _p, _p]),
     "pglb_head_dots_x16": (c_int, [_p, _i64, _i64, _i64, _i64, c_int, _p, _p, _p, _p, _p]),
+    "pglb_gat_fused_train_drop_csr_f32": (c_int, [_p, _p, _p, _i64, _p, _p, ctypes.c_float, _p, _i64, _p, _i64, _i64,
+                                                  _i64, _i64, _i64, ctypes.c_float, _u64, _u64, _p, c_size_t, _p]),
+    "pglb_gat_fused_train_drop_csr_x16": (c_int, [_p, _p, _p, _i64, _p, _p, ctypes.c_float, _p, _i64, _p, _i64, _i64,
+                                                  _i64, _i64, _i64, c_int, ctypes.c_float, _u64, _u64, _p, c_size_t,
+                                                  _p]),
+    "pglb_gat_bwd_edge_drop_f32": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _p, _p, ctypes.c_float,
+                                           _i64, _i64, _i64, ctypes.c_float, _u64, _u64, _p, _p, _p]),
+    "pglb_gat_bwd_edge_drop_x16": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _p, _p, ctypes.c_float,
+                                           _i64, _i64, _i64, c_int, ctypes.c_float, _u64, _u64, _p, _p, _p]),
+    "pglb_attn_dropout_keep_host": (c_int, [_u64, _u64, ctypes.c_float, _i64, _i64, _i64, _p]),
     "pglb_gat_attention_csr_f32": (c_int, [_p, _p, _p, _p, ctypes.c_float, _p, _i64, _i64, _i64, _p,
                                            c_size_t, _p]),
     "pglb_sddmm_dot_f32": (c_int, [_p, _p, _p, _i64, _p, _i64, _i64, _i64, _i64, _p, _p]),

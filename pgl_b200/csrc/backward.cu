@@ -111,13 +111,17 @@ __global__ void __launch_bounds__(256) maxmin_bwd_kernel(const int64_t *__restri
 // lanes form a head; four gathered feature rows are in flight per lane before the first dot product.
 // T: element type of f, g and out (float, or the 16-bit type of pglb_gat_bwd_edge_x16: a lane reads 8 bytes and widens
 // them exactly, and the arithmetic after that is the float32 kernel's).  a_s, a_d, lse, alpha_e and dz_e are fp32.
-template <int LPH, typename T>
+// DROP (attention dropout, pglb_gat_bwd_edge_drop_*): the forward was out = sum beta f[src] with beta = s m alpha
+// (m = the keep bit of the slot and head, s = 1 / (1 - p)).  Then d alpha = s m <G, f[src]>, sum_k alpha_k d alpha_k
+// = <G, out> is still delta, and the edge kernel writes beta in place of alpha (what grad f is aggregated with).  Each
+// lane recomputes its own slot's keep word; the consume loop shuffles it along with the slot's row and edge id.
+template <int LPH, typename T, bool DROP>
 __global__ void __launch_bounds__(256) gat_bwd_edge_kernel(
     const int64_t *__restrict__ rows, const int64_t *__restrict__ cols, const int64_t *__restrict__ eid,
     const T *__restrict__ f, int64_t ldf, const T *__restrict__ g, int64_t ldg,
     const T *__restrict__ out, int64_t ldo, const float *__restrict__ a_s, const float *__restrict__ a_d,
     const float *__restrict__ lse, float slope, int64_t E, int H, int D, float *__restrict__ alpha_e,
-    float *__restrict__ dz_e) {
+    float *__restrict__ dz_e, const AttnDrop drop) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -138,6 +142,8 @@ __global__ void __launch_bounds__(256) gat_bwd_edge_kernel(
         const long long r_l = in ? ld_stream(rows + j) : 0;
         const long long c_l = in ? ld_stream(cols + j) : 0;
         const long long i_l = in ? (eid ? ld_stream(eid + j) : j) : 0;
+        unsigned kw_l = 0;
+        if constexpr (DROP) kw_l = attn_keep_word(drop, (uint64_t)j, H);
         const int cnt = (E - base) < 32 ? (int)(E - base) : 32;
         long long cur = -1;
         float4 g4 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -146,12 +152,14 @@ __global__ void __launch_bounds__(256) gat_bwd_edge_kernel(
             float4 fv[4];
             float as[4];
             long long rr[4], ii[4];
+            unsigned kk[4];
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
                 const int k = (k0 + u) & 31;
                 const long long cc = __shfl_sync(0xffffffffu, c_l, k);
                 rr[u] = __shfl_sync(0xffffffffu, r_l, k);
                 ii[u] = __shfl_sync(0xffffffffu, i_l, k);
+                if constexpr (DROP) kk[u] = __shfl_sync(0xffffffffu, kw_l, k);
                 fv[u] = make_float4(0.f, 0.f, 0.f, 0.f);
                 as[u] = 0.f;
                 if (k0 + u < cnt && act) {
@@ -174,13 +182,19 @@ __global__ void __launch_bounds__(256) gat_bwd_edge_kernel(
                     }
                     delta = head_sum(d);
                 }
-                const float da = head_sum(dot4(fv[u], g4));
+                float da = head_sum(dot4(fv[u], g4));
                 const float z = as[u] + ad;
                 const bool pos = z > 0.0f;   // leaky_relu'(0) = slope, the convention of the framework's LeakyReLU backward
                 const float alpha = expf((pos ? z : z * slope) - ls);
+                float beta = alpha;
+                if constexpr (DROP) {
+                    const bool keep = (kk[u] >> head) & 1u;
+                    da = keep ? drop.scale * da : 0.f;
+                    beta = keep ? alpha * drop.scale : 0.f;
+                }
                 const float dl = alpha * (da - delta);
                 if (lead) {
-                    alpha_e[ii[u] * H + head] = alpha;
+                    alpha_e[ii[u] * H + head] = beta;
                     dz_e[ii[u] * H + head] = pos ? dl : dl * slope;
                 }
             }
@@ -242,12 +256,13 @@ extern "C" int pglb_edge_softmax_bwd_csr_f32(const int64_t *indptr, const int64_
 
 // The checks and the launch of both edge-backward entries.  T: element type of f, grad_out and out; their rows are
 // 16-byte aligned (ld * sizeof(T) % 16 == 0) for either type.
+// drop (nullable): the attention-dropout stream of the DROP kernel (H % 4 == 0 and H <= 32 then).
 template <typename T>
 static int gat_bwd_edge_entry(const char *name, const int64_t *rows, const int64_t *cols, const int64_t *eid,
                               const void *f_, int64_t ldf, const void *grad_out_, int64_t ldg, const void *out_,
                               int64_t ldo, const float *attn_src, const float *attn_dst, const float *lse,
                               float negative_slope, int64_t num_edges, int64_t H, int64_t head_dim, float *alpha_e,
-                              float *dz_e, void *stream_) {
+                              float *dz_e, void *stream_, const AttnDrop *drop = nullptr) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     const T *f = reinterpret_cast<const T *>(f_), *grad_out = reinterpret_cast<const T *>(grad_out_),
             *out = reinterpret_cast<const T *>(out_);
@@ -257,6 +272,7 @@ static int gat_bwd_edge_entry(const char *name, const int64_t *rows, const int64
     const int64_t lph = head_dim / 4;
     PGLB_CHECK_ARG(D <= 128 && head_dim % 4 == 0 && (lph & (lph - 1)) == 0, PGLB_EUNSUPPORTED,
                    "%s: needs H*head_dim <= 128 and head_dim in {4, 8, 16, 32, 64, 128}", name);
+    PGLB_CHECK_ARG(!drop || H % 4 == 0, PGLB_EUNSUPPORTED, "%s: needs H %% 4 == 0", name);
     if (num_edges == 0) return PGLB_OK;
     PGLB_CHECK_ARG(rows && cols && f && grad_out && out && attn_src && attn_dst && lse && alpha_e && dz_e, PGLB_EINVAL,
                    "%s: NULL pointer", name);
@@ -266,9 +282,18 @@ static int gat_bwd_edge_entry(const char *name, const int64_t *rows, const int64
                    PGLB_ESHAPE, "%s: rows must be 16-byte aligned", name);
     const int grid = grid_of(num_edges * 1, 64);  // a warp per 32 slots, grid-stride
 #define PGLB_GBE(L)                                                                                                   \
-    gat_bwd_edge_kernel<L, T><<<grid, 256, 0, stream>>>(rows, cols, eid, f, ldf, grad_out, ldg, out, ldo, attn_src,   \
-                                                       attn_dst, lse, negative_slope, num_edges, (int)H, (int)D,     \
-                                                       alpha_e, dz_e)
+    do {                                                                                                              \
+        if (drop)                                                                                                     \
+            gat_bwd_edge_kernel<L, T, true><<<grid, 256, 0, stream>>>(rows, cols, eid, f, ldf, grad_out, ldg, out,    \
+                                                                      ldo, attn_src, attn_dst, lse, negative_slope,   \
+                                                                      num_edges, (int)H, (int)D, alpha_e, dz_e,       \
+                                                                      *drop);                                         \
+        else                                                                                                          \
+            gat_bwd_edge_kernel<L, T, false><<<grid, 256, 0, stream>>>(rows, cols, eid, f, ldf, grad_out, ldg, out,   \
+                                                                       ldo, attn_src, attn_dst, lse, negative_slope,  \
+                                                                       num_edges, (int)H, (int)D, alpha_e, dz_e,      \
+                                                                       AttnDrop{});                                   \
+    } while (0)
     switch ((int)lph) {
         case 1: PGLB_GBE(1); break;
         case 2: PGLB_GBE(2); break;
@@ -306,6 +331,55 @@ extern "C" int pglb_gat_bwd_edge_x16(const int64_t *rows, const int64_t *cols, c
     return gat_bwd_edge_entry<__half>("pglb_gat_bwd_edge_x16", rows, cols, eid, f, ldf, grad_out, ldg, out, ldo,
                                       attn_src, attn_dst, lse, negative_slope, num_edges, H, head_dim, alpha_e, dz_e,
                                       stream_);
+}
+
+// Edge backward with attention dropout (include/pglb.h): the edge entries' arguments plus attn_drop, seed, offset,
+// which are checked first, before any CUDA call.
+extern "C" int pglb_gat_bwd_edge_drop_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *f,
+                                          int64_t ldf, const float *grad_out, int64_t ldg, const float *out,
+                                          int64_t ldo, const float *attn_src, const float *attn_dst, const float *lse,
+                                          float negative_slope, int64_t num_edges, int64_t H, int64_t head_dim,
+                                          float attn_drop, uint64_t seed, uint64_t offset, float *alpha_e,
+                                          float *dz_e, void *stream_) {
+    const char *name = "pglb_gat_bwd_edge_drop_f32";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    return gat_bwd_edge_entry<float>(name, rows, cols, eid, f, ldf, grad_out, ldg, out, ldo, attn_src, attn_dst, lse,
+                                     negative_slope, num_edges, H, head_dim, alpha_e, dz_e, stream_, &drop);
+}
+
+extern "C" int pglb_gat_bwd_edge_drop_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *f,
+                                          int64_t ldf, const void *grad_out, int64_t ldg, const void *out,
+                                          int64_t ldo, const float *attn_src, const float *attn_dst, const float *lse,
+                                          float negative_slope, int64_t num_edges, int64_t H, int64_t head_dim,
+                                          int dtype, float attn_drop, uint64_t seed, uint64_t offset, float *alpha_e,
+                                          float *dz_e, void *stream_) {
+    const char *name = "pglb_gat_bwd_edge_drop_x16";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    if (dtype == PGLB_DTYPE_BF16)
+        return gat_bwd_edge_entry<__nv_bfloat16>(name, rows, cols, eid, f, ldf, grad_out, ldg, out, ldo, attn_src,
+                                                 attn_dst, lse, negative_slope, num_edges, H, head_dim, alpha_e, dz_e,
+                                                 stream_, &drop);
+    return gat_bwd_edge_entry<__half>(name, rows, cols, eid, f, ldf, grad_out, ldg, out, ldo, attn_src, attn_dst, lse,
+                                      negative_slope, num_edges, H, head_dim, alpha_e, dz_e, stream_, &drop);
+}
+
+// The keep words of dst-CSR slots slot0 .. slot0 + n_slots - 1 on the host (include/pglb.h): the same attn_keep_word
+// the kernels call, so a test can pin the dropout stream without a GPU.
+extern "C" int pglb_attn_dropout_keep_host(uint64_t seed, uint64_t offset, float attn_drop, int64_t slot0,
+                                           int64_t n_slots, int64_t H, uint32_t *keep_words) {
+    const char *name = "pglb_attn_dropout_keep_host";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    PGLB_CHECK_ARG(slot0 >= 0 && n_slots >= 0, PGLB_EINVAL, "%s: bad slot range", name);
+    PGLB_CHECK_ARG(H > 0 && H <= 32 && H % 4 == 0, PGLB_EUNSUPPORTED, "%s: needs H %% 4 == 0 and H <= 32", name);
+    if (n_slots == 0) return PGLB_OK;
+    PGLB_CHECK_ARG(keep_words != nullptr, PGLB_EINVAL, "%s: NULL pointer", name);
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    for (int64_t i = 0; i < n_slots; ++i) keep_words[i] = attn_keep_word(drop, (uint64_t)(slot0 + i), (int)H);
+    return PGLB_OK;
 }
 
 extern "C" int pglb_maxmin_bwd_f32(const int64_t *src_indptr, const int64_t *dst_of_slot,

@@ -3,6 +3,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 #include <stdio.h>
 
@@ -114,6 +115,77 @@ template <typename T>
 __device__ __forceinline__ float4 ldg_row4(const T *p) {
     if constexpr (sizeof(T) == 4) return __ldg(reinterpret_cast<const float4 *>(p));
     else return widen4<T>(__ldg(reinterpret_cast<const uint2 *>(p)));
+}
+
+// ---- attention dropout of the fused GAT training path (the *_drop_* entries) ----------------------------------------
+// The keep decision of dst-CSR slot j (absolute slot index) and head h, for drop probability p:
+//   draw = Philox4x32-10(counter = (j lo32, j hi32, h / 4, offset / 4), key = (seed lo32, seed hi32)) word h % 4
+//   kept iff draw >= thresh,  thresh = min(floor(p * 2^32), 2^32 - 1);  a kept weight is scaled by s = 1 / (1 - p)
+// (Philox: Salmon, Moraes, Dror, Shaw, "Parallel random numbers: as easy as 1, 2, 3", SC 2011).  attn_keep_word is the
+// only statement of this rule: the forward kernel, the backward edge kernel and pglb_attn_dropout_keep_host call it,
+// so the forward and the backward recompute the same mask in registers and no [E, H] mask exists.
+struct AttnDrop {
+    uint64_t seed;
+    uint32_t ctr3;     // offset / 4: counter word 3
+    uint32_t thresh;   // kept iff draw >= thresh
+    float scale;       // s = (float)(1 / (1 - p))
+};
+
+// the argument checks every attention-dropout entry makes before anything else: 0 < p < 1 (NaN fails), offset % 4 == 0
+inline int attn_drop_check(const char *name, float p, uint64_t offset) {
+    PGLB_CHECK_ARG(p > 0.0f && p < 1.0f, PGLB_EINVAL, "%s: attn_drop must lie in (0, 1)", name);
+    PGLB_CHECK_ARG(offset % 4 == 0, PGLB_EINVAL, "%s: offset must be a multiple of 4", name);
+    return PGLB_OK;
+}
+
+// thresh and s derived in double from the float p an entry receives (after attn_drop_check)
+inline AttnDrop attn_drop_of(float p, uint64_t seed, uint64_t offset) {
+    AttnDrop d;
+    const double t = floor((double)p * 4294967296.0);
+    d.seed = seed;
+    d.ctr3 = (uint32_t)(offset / 4);
+    d.thresh = t >= 4294967295.0 ? 0xffffffffu : (uint32_t)t;
+    d.scale = (float)(1.0 / (1.0 - (double)p));
+    return d;
+}
+
+__host__ __device__ __forceinline__ uint32_t mulhilo32(uint32_t a, uint32_t b, uint32_t *hi) {
+#ifdef __CUDA_ARCH__
+    *hi = __umulhi(a, b);
+    return a * b;
+#else
+    const uint64_t m = (uint64_t)a * b;
+    *hi = (uint32_t)(m >> 32);
+    return (uint32_t)m;
+#endif
+}
+
+__host__ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        if (r) {
+            k0 += 0x9E3779B9u;
+            k1 += 0xBB67AE85u;
+        }
+        uint32_t hi0, hi1;
+        const uint32_t lo0 = mulhilo32(0xD2511F53u, c.x, &hi0);
+        const uint32_t lo1 = mulhilo32(0xCD9E8D57u, c.z, &hi1);
+        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+    }
+    return c;
+}
+
+// keep word of slot j: bit h = head h kept (H % 4 == 0, H <= 32: one Philox call per four heads)
+__host__ __device__ __forceinline__ uint32_t attn_keep_word(const AttnDrop &d, uint64_t j, int H) {
+    uint32_t w = 0;
+    for (int q = 0; q < H / 4; ++q) {
+        const uint4 r = philox4x32_10(make_uint4((uint32_t)j, (uint32_t)(j >> 32), (uint32_t)q, d.ctr3),
+                                      (uint32_t)d.seed, (uint32_t)(d.seed >> 32));
+        const uint32_t b = (uint32_t)(r.x >= d.thresh) | ((uint32_t)(r.y >= d.thresh) << 1) |
+                           ((uint32_t)(r.z >= d.thresh) << 2) | ((uint32_t)(r.w >= d.thresh) << 3);
+        w |= b << (4 * q);
+    }
+    return w;
 }
 
 }  // namespace pglb

@@ -480,8 +480,8 @@ int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, 
 template <typename T>
 int gat_fused_run(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf, void *out,
                   int64_t ldo, int64_t n_dst, int64_t n_src, int64_t E, int64_t D, int64_t H,
-                  const float *attn_src, const float *attn_dst, float slope, float *lse, void *ws, size_t ws_bytes,
-                  cudaStream_t stream);
+                  const float *attn_src, const float *attn_dst, float slope, float *lse, const AttnDrop *drop, void *ws,
+                  size_t ws_bytes, cudaStream_t stream);
 template <typename T>
 bool gat5_takes(int64_t D, float slope, const void *f, int64_t ldf, const float *attn_src, int64_t H, int64_t n_src);
 
@@ -751,7 +751,7 @@ template <typename T>
 static int gat_fused_entry(const char *name, const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
                            const float *attn_src, const float *attn_dst, float negative_slope, void *out, int64_t ldo,
                            float *lse, int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H, int64_t head_dim,
-                           void *ws, size_t ws_bytes, void *stream_) {
+                           void *ws, size_t ws_bytes, void *stream_, const AttnDrop *drop = nullptr) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     constexpr int64_t B = sizeof(T);
     PGLB_CHECK_ARG(n_dst >= 0 && n_src >= 0 && num_edges >= 0 && H > 0 && head_dim > 0, PGLB_EINVAL, "%s: bad size", name);
@@ -778,7 +778,7 @@ static int gat_fused_entry(const char *name, const int64_t *indptr, const int64_
     PGLB_CHECK_ARG(ws && (reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
                    "%s: workspace NULL or not 256-byte aligned", name);
     return gat_fused_run<T>(indptr, cols, f, ldf, out, ldo, n_dst, n_src, num_edges, D, H, attn_src, attn_dst,
-                            negative_slope, lse, ws, ws_bytes, stream);
+                            negative_slope, lse, drop, ws, ws_bytes, stream);
 }
 
 extern "C" int pglb_gat_fused_csr_f32(const int64_t *indptr, const int64_t *cols, const float *f,
@@ -832,6 +832,42 @@ extern "C" int pglb_gat_fused_train_csr_x16(const int64_t *indptr, const int64_t
         return gat_fused_entry<T>("pglb_gat_fused_train_csr_x16", indptr, cols, f, ldf, attn_src, attn_dst,
                                   negative_slope, out, ldo, lse, n_dst, n_src, num_edges, H, head_dim, ws, ws_bytes,
                                   stream_);
+    };
+    return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
+}
+
+// Training forward with attention dropout (include/pglb.h): the train entries' arguments plus attn_drop, seed, offset.
+// The dropout arguments are checked first, before any CUDA call.
+extern "C" int pglb_gat_fused_train_drop_csr_f32(const int64_t *indptr, const int64_t *cols, const float *f,
+                                                 int64_t ldf, const float *attn_src, const float *attn_dst,
+                                                 float negative_slope, float *out, int64_t ldo, float *lse,
+                                                 int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H,
+                                                 int64_t head_dim, float attn_drop, uint64_t seed, uint64_t offset,
+                                                 void *ws, size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_gat_fused_train_drop_csr_f32";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    PGLB_CHECK_ARG(lse != nullptr || n_dst == 0, PGLB_EINVAL, "%s: NULL lse", name);
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    return gat_fused_entry<float>(name, indptr, cols, f, ldf, attn_src, attn_dst, negative_slope, out, ldo, lse, n_dst,
+                                  n_src, num_edges, H, head_dim, ws, ws_bytes, stream_, &drop);
+}
+
+extern "C" int pglb_gat_fused_train_drop_csr_x16(const int64_t *indptr, const int64_t *cols, const void *f,
+                                                 int64_t ldf, const float *attn_src, const float *attn_dst,
+                                                 float negative_slope, void *out, int64_t ldo, float *lse,
+                                                 int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H,
+                                                 int64_t head_dim, int dtype, float attn_drop, uint64_t seed,
+                                                 uint64_t offset, void *ws, size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_gat_fused_train_drop_csr_x16";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    PGLB_CHECK_ARG(lse != nullptr || n_dst == 0, PGLB_EINVAL, "%s: NULL lse", name);
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    auto run = [&](auto *elem) -> int {
+        using T = std::remove_pointer_t<decltype(elem)>;
+        return gat_fused_entry<T>(name, indptr, cols, f, ldf, attn_src, attn_dst, negative_slope, out, ldo, lse, n_dst,
+                                  n_src, num_edges, H, head_dim, ws, ws_bytes, stream_, &drop);
     };
     return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
 }

@@ -756,9 +756,10 @@ __global__ void __launch_bounds__(256) spmm_stream_fixup_kernel(const StreamP p)
 
 // Fused-GAT fix-up: merge the (acc, m, l) partials of a cut row: M = max m_i,
 // out = sum_i acc_i e^{m_i - M} / sum_i l_i e^{m_i - M}.  The partials are fp32; TO is the element type of out (a
-// 16-bit out is rounded once, on the store).
-template <typename TO>
-__global__ void __launch_bounds__(256) spmm_stream_fixup_gat_kernel(const StreamP p) {
+// 16-bit out is rounded once, on the store).  DROP (attention dropout): the acc partials hold only the kept slots and
+// the quotient is multiplied by drop_scale = 1 / (1 - p).
+template <typename TO, bool DROP>
+__global__ void __launch_bounds__(256) spmm_stream_fixup_gat_kernel(const StreamP p, float drop_scale) {
     const int lane = threadIdx.x & 31;
     const int64_t t = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (t >= p.ntasks) return;
@@ -783,6 +784,9 @@ __global__ void __launch_bounds__(256) spmm_stream_fixup_gat_kernel(const Stream
     for (int64_t u = t + 1; u < u_end; ++u) add(2 * u);
     acc.x = __fdiv_rn(acc.x, L); acc.y = __fdiv_rn(acc.y, L);
     acc.z = __fdiv_rn(acc.z, L); acc.w = __fdiv_rn(acc.w, L);
+    if constexpr (DROP) {
+        acc.x *= drop_scale; acc.y *= drop_scale; acc.z *= drop_scale; acc.w *= drop_scale;
+    }
     if constexpr (sizeof(TO) == 4)
         *reinterpret_cast<float4 *>(p.out + r * p.ldo + c) = acc;
     else
@@ -958,7 +962,7 @@ static int launch_stream128(const StreamP &p, cudaStream_t stream) {
     PGLB_LAUNCH_CHECK("spmm_stream128_kernel");
     const int64_t fblocks = (p.ntasks * 32 + 255) / 256;
     if (YM == 2) {
-        spmm_stream_fixup_gat_kernel<float><<<(unsigned)fblocks, 256, 0, stream>>>(p);
+        spmm_stream_fixup_gat_kernel<float, false><<<(unsigned)fblocks, 256, 0, stream>>>(p, 1.0f);
     } else {
         spmm_stream_fixup_kernel<float, 1, RK><<<(unsigned)fblocks, 256, 0, stream>>>(p);
     }
@@ -1205,12 +1209,12 @@ bool gat5_takes(int64_t D, float slope, const void *f, int64_t ldf, const float 
 
 // Single-pass GAT aggregation (inference): out[d,h,:] = sum_j softmax_j(leaky(as[src_j,h] + ad[d,h])) f[src_j,h,:].
 // T: element type of f and out.  float32 calls outside gat5 take spmm_stream128_kernel<YM = 2>; a 16-bit call must be
-// one gat5 takes.
+// one gat5 takes.  drop (nullable, training only: lse non-NULL): the attention-dropout stream of the DROP kernels.
 template <typename T>
 int gat_fused_run(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf, void *out,
                   int64_t ldo, int64_t n_dst, int64_t n_src, int64_t E, int64_t D, int64_t H,
-                  const float *attn_src, const float *attn_dst, float slope, float *lse, void *ws, size_t ws_bytes,
-                  cudaStream_t stream) {
+                  const float *attn_src, const float *attn_dst, float slope, float *lse, const AttnDrop *drop, void *ws,
+                  size_t ws_bytes, cudaStream_t stream) {
     // the row statistics are written by spmm_gat5_kernel and the merge kernel only
     const bool tma = gat5_eligible<T>(D, slope, f, ldf, attn_src, H, n_src);
     PGLB_CHECK_ARG(!lse || tma, PGLB_EUNSUPPORTED,
@@ -1236,7 +1240,8 @@ int gat_fused_run(const int64_t *indptr, const int64_t *cols, const void *f, int
         const int rc = launch_empty_rows<T>(p, stream);
         if (rc) return rc;
     }
-    if (tma) return launch_gat5<T>(p, attn_src, H, stream);
+    if (tma && drop) return launch_gat5<T, true>(p, attn_src, H, *drop, stream);
+    if (tma) return launch_gat5<T, false>(p, attn_src, H, AttnDrop{}, stream);
     if constexpr (sizeof(T) == 4) return launch_stream128<0, false, 0, 2>(p, stream);
     return PGLB_EUNSUPPORTED;   // not reached: refused above
 }

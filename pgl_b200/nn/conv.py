@@ -224,12 +224,13 @@ class GATConv(nn.Module):
                 output = self.activation(output)
             return output
         output = None
-        if no_attn_drop and type(graph).__name__ == "Graph" and feature.dtype in _FUSED_TRAIN_DTYPES:
-            # training without attention dropout: the same single-pass kernel, which keeps the rows' log-sum-exp, and
-            # a fused backward (ops._GatFused); None when the shape is outside it
+        if type(graph).__name__ == "Graph" and feature.dtype in _FUSED_TRAIN_DTYPES:
+            # training: the same single-pass kernel, which keeps the rows' log-sum-exp, and a fused backward
+            # (ops._GatFused), with the attention dropout inside both; None when the shape is outside them
             from .. import ops
             output = ops.gat_fused_train(graph._fwd_csr(), graph._bwd_csr, feature, attn_src, attn_dst,
-                                         self.leaky_relu.negative_slope, out_dtype=out_dtype)
+                                         self.leaky_relu.negative_slope, out_dtype=out_dtype,
+                                         attn_drop=0.0 if no_attn_drop else self.attn_drop)
         if output is None:
             attn_src, attn_dst = unfused_attn()
             alpha = graph.send_uv(attn_src, attn_dst, "add")

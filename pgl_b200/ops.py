@@ -1312,10 +1312,12 @@ class _GatFused(torch.autograd.Function):
     four ops).  Forward = pglb_gat_fused_train_csr_f32 (one launch; keeps only lse[N, H]).  Backward = one edge kernel
     (pglb_gat_bwd_edge_f32: alpha rebuilt, SDDMM dot, softmax and LeakyReLU backward) + three reverse-CSR aggregations
     on the existing kernels.  16-bit f2: the *_x16 entries; out and grad f in f2's dtype, lse, alpha, dz and the
-    attention and its gradients float32 (a_s / a_d are float32 here)."""
+    attention and its gradients float32 (a_s / a_d are float32 here).  drop = (p, seed, offset): attention dropout on
+    the *_drop_* entries, which recompute the keep mask from (seed, offset) in the forward and in the backward; the
+    edge kernel then returns the dropped attention, with which grad f is aggregated as before."""
 
     @staticmethod
-    def forward(ctx, f2, a_s, a_d, fwd, bwd, slope, H, Dh):
+    def forward(ctx, f2, a_s, a_d, fwd, bwd, slope, H, Dh, drop=None):
         n = int(f2.shape[0])
         E = int(fwd["cols"].shape[0])
         n_dst = int(fwd["indptr"].shape[0]) - 1
@@ -1325,7 +1327,16 @@ class _GatFused(torch.autograd.Function):
         check(lib.pglb_spmm_csr_ws(n_dst, E, H * Dh, ctypes.byref(need)))
         ws = workspace(f2.device, need.value)
         with torch.cuda.device(f2.device):
-            if f2.dtype in HALF_DTYPES:
+            if drop is not None and f2.dtype in HALF_DTYPES:
+                check(lib.pglb_gat_fused_train_drop_csr_x16(
+                    _ptr(fwd["indptr"]), _ptr(fwd["cols"]), _ptr(f2), f2.stride(0), _ptr(a_s), _ptr(a_d), float(slope),
+                    _ptr(out), out.stride(0), _ptr(lse), n_dst, n, E, H, Dh, _DTYPE16[f2.dtype], *drop, _ptr(ws),
+                    ws.numel(), _stream()))
+            elif drop is not None:
+                check(lib.pglb_gat_fused_train_drop_csr_f32(
+                    _ptr(fwd["indptr"]), _ptr(fwd["cols"]), _ptr(f2), f2.stride(0), _ptr(a_s), _ptr(a_d), float(slope),
+                    _ptr(out), out.stride(0), _ptr(lse), n_dst, n, E, H, Dh, *drop, _ptr(ws), ws.numel(), _stream()))
+            elif f2.dtype in HALF_DTYPES:
                 check(lib.pglb_gat_fused_train_csr_x16(
                     _ptr(fwd["indptr"]), _ptr(fwd["cols"]), _ptr(f2), f2.stride(0), _ptr(a_s), _ptr(a_d), float(slope),
                     _ptr(out), out.stride(0), _ptr(lse), n_dst, n, E, H, Dh, _DTYPE16[f2.dtype], _ptr(ws), ws.numel(),
@@ -1334,13 +1345,13 @@ class _GatFused(torch.autograd.Function):
                 check(lib.pglb_gat_fused_train_csr_f32(
                     _ptr(fwd["indptr"]), _ptr(fwd["cols"]), _ptr(f2), f2.stride(0), _ptr(a_s), _ptr(a_d), float(slope),
                     _ptr(out), out.stride(0), _ptr(lse), n_dst, n, E, H, Dh, _ptr(ws), ws.numel(), _stream()))
-        ctx.meta = (fwd, bwd, float(slope), H, Dh)
+        ctx.meta = (fwd, bwd, float(slope), H, Dh, drop)
         ctx.save_for_backward(f2, a_s, a_d, out, lse)
         return out
 
     @staticmethod
     def backward(ctx, g):
-        fwd, bwd, slope, H, Dh = ctx.meta
+        fwd, bwd, slope, H, Dh, drop = ctx.meta
         bwd = bwd() if callable(bwd) else bwd
         f2, a_s, a_d, out, lse = ctx.saved_tensors
         half = f2.dtype in HALF_DTYPES
@@ -1350,7 +1361,17 @@ class _GatFused(torch.autograd.Function):
         alpha = torch.empty((E, H), dtype=torch.float32, device=g.device)
         dz = torch.empty((E, H), dtype=torch.float32, device=g.device)
         with torch.cuda.device(g.device):
-            if half:
+            if drop is not None and half:
+                check(lib.pglb_gat_bwd_edge_drop_x16(_ptr(fwd["rows"]), _ptr(fwd["cols"]), _ptr(fwd["eid"]), _ptr(f2),
+                                                     f2.stride(0), _ptr(g), g.stride(0), _ptr(out), out.stride(0),
+                                                     _ptr(a_s), _ptr(a_d), _ptr(lse), slope, E, H, Dh,
+                                                     _DTYPE16[f2.dtype], *drop, _ptr(alpha), _ptr(dz), _stream()))
+            elif drop is not None:
+                check(lib.pglb_gat_bwd_edge_drop_f32(_ptr(fwd["rows"]), _ptr(fwd["cols"]), _ptr(fwd["eid"]), _ptr(f2),
+                                                     f2.stride(0), _ptr(g), g.stride(0), _ptr(out), out.stride(0),
+                                                     _ptr(a_s), _ptr(a_d), _ptr(lse), slope, E, H, Dh, *drop,
+                                                     _ptr(alpha), _ptr(dz), _stream()))
+            elif half:
                 check(lib.pglb_gat_bwd_edge_x16(_ptr(fwd["rows"]), _ptr(fwd["cols"]), _ptr(fwd["eid"]), _ptr(f2),
                                                 f2.stride(0), _ptr(g), g.stride(0), _ptr(out), out.stride(0),
                                                 _ptr(a_s), _ptr(a_d), _ptr(lse), slope, E, H, Dh, _DTYPE16[f2.dtype],
@@ -1361,33 +1382,53 @@ class _GatFused(torch.autograd.Function):
                                                 _ptr(a_s), _ptr(a_d), _ptr(lse), slope, E, H, Dh, _ptr(alpha),
                                                 _ptr(dz), _stream()))
         gf = gs = gd = None
-        if ctx.needs_input_grad[0]:   # grad f[s] = sum over the out-edges of s of alpha[e] * g[dst[e]]
+        # grad f[s] = sum over the out-edges of s of alpha[e] * g[dst[e]] (with dropout: the dropped attention)
+        if ctx.needs_input_grad[0]:
             gf = _spmm_raw(bwd["indptr"], bwd["cols"], g, n_src, "sum", eid=bwd["eid"], y2=alpha, y_bcast=BCAST_HEAD,
                            head_dim=Dh, msg_op="mul", max_degree=bwd.get("max_degree", -1))
         if ctx.needs_input_grad[1]:   # z = as[src] + ad[dst]: send_uv(add)'s backward
             gs = _spmm_raw(bwd["indptr"], bwd["eid"], dz, n_src, "sum", max_degree=bwd.get("max_degree", -1))
         if ctx.needs_input_grad[2]:
             gd = _spmm_raw(fwd["indptr"], fwd["eid"], dz, n_dst, "sum", max_degree=fwd.get("max_degree", -1))
-        return gf, gs, gd, None, None, None, None, None
+        return gf, gs, gd, None, None, None, None, None, None
 
 
 GAT_FUSED_TRAIN = os.environ.get("PGLB_GAT_FUSED_TRAIN", "1") != "0"
 
 
-def gat_fused_train(fwd, bwd, f, attn_src, attn_dst, negative_slope=0.2, out_dtype=None):
+def _attn_drop_stream(device):
+    """(seed, offset) of one attention-dropout call from the default CUDA generator of ``device``: its seed and its
+    current offset, which then advances by 4, so every call draws a fresh mask and torch.manual_seed replays a
+    sequence of calls bit for bit."""
+    gen = torch.cuda.default_generators[device.index if device.index is not None else torch.cuda.current_device()]
+    seed, offset = int(gen.initial_seed()), int(gen.get_offset())
+    gen.set_offset(offset + 4)
+    return seed, offset
+
+
+def gat_fused_train(fwd, bwd, f, attn_src, attn_dst, negative_slope=0.2, out_dtype=None, attn_drop=0.0, seed=None):
     """gat_fused with a backward.  f [N, H, Dh], 64 < H*Dh <= 128, H % 4 == 0, Dh a power of two >= 4,
     0 <= slope <= 1; returns [N, H, Dh], or None when the shape is outside the fused kernels (the caller keeps the
     op-by-op path).  ``bwd`` is the reverse CSR dict or a callable returning it.
     The result dtype is ``out_dtype``, or by default torch's promotion of f's and the attention's dtypes.  float32 f
     runs the float32 kernels (the result cast to the result dtype).  bfloat16 / float16 f runs the 16-bit kernels when
     the result dtype is f's (attention widened to float32; grad f in f's dtype, grad attention formed in float32 and
-    returned in the attention's dtype); other 16-bit calls return None."""
+    returned in the attention's dtype); other 16-bit calls return None.
+    ``attn_drop`` in (0, 1): dropout on the normalised attention, per edge and head, inside the same kernels (the
+    *_drop_* entries of include/pglb.h).  The mask comes from ``seed`` = (seed, offset), offset a multiple of 4, or by
+    default from the default CUDA generator of f's device (whose offset then advances by 4).  attn_drop >= 1 and calls
+    during a CUDA graph capture return None (the caller keeps the op-by-op path with its own dropout)."""
     require_cuda(f, attn_src, attn_dst)
     n, H, Dh = int(f.shape[0]), int(f.shape[1]), int(f.shape[2])
     half = f.dtype in HALF_DTYPES
     res = _result_dtype(out_dtype, f, attn_src, attn_dst)
     if not GAT_FUSED_TRAIN or H * Dh > 128 or H * Dh <= 64 or H % 4 or H > 32:
         return None
+    attn_drop = float(attn_drop)
+    if not 0.0 <= attn_drop < 1.0:
+        return None
+    if attn_drop > 0.0 and torch.cuda.is_current_stream_capturing():
+        return None     # the generator's offset advances on the host: not replayable by a graph
     if not (f.dtype == torch.float32 or (half and res == f.dtype and torch.float64 not in (attn_src.dtype,
                                                                                           attn_dst.dtype))):
         return None
@@ -1400,8 +1441,11 @@ def gat_fused_train(fwd, bwd, f, attn_src, attn_dst, negative_slope=0.2, out_dty
     a_s, a_d = (_att32(attn_src), _att32(attn_dst)) if half else (_f32_2d(attn_src), _f32_2d(attn_dst))
     if f2.data_ptr() % 16 or (f2.stride(0) * f2.element_size()) % 16 or a_s.data_ptr() % 16:
         return None
+    drop = None
+    if attn_drop > 0.0:
+        drop = (attn_drop,) + (tuple(int(v) for v in seed) if seed is not None else _attn_drop_stream(f2.device))
     try:
-        out = _GatFused.apply(f2, a_s, a_d, fwd, bwd, float(negative_slope), H, Dh)
+        out = _GatFused.apply(f2, a_s, a_d, fwd, bwd, float(negative_slope), H, Dh, drop)
     except _lib.PglbError as ex:
         if ex.code == -4:   # PGLB_EUNSUPPORTED: e.g. 32 heads, whose attention rows do not fit the kernel's rings
             return None
