@@ -435,6 +435,41 @@ int pglb_reindex_graph(const int64_t *x, int64_t n, const int64_t *neighbors, co
                        int64_t m, int64_t *table, int64_t *reindex_src, int64_t *reindex_dst,
                        int64_t *out_nodes, int64_t *num_out, void *ws, size_t ws_bytes, void *stream);
 
+/* ------------------------------------------------------------------------------------
+ * Random walks (csrc/walk.cu).  Replace pgl.sampling.random_walk / node2vec_walk / node2vec_walk_plus
+ * (pgl/sampling/walk.py:23-183, graph_kernel.pyx:142-224) on the src-keyed CSR (indptr = adj_src_index._indptr,
+ * cols = adj_src_index._sorted_v): one walker per thread, the whole walk in one launch.
+ *   - Walker i starts at nodes[i] and writes row i of out (row-major, L columns): the walk, then -1 after it ends.
+ *     A walk ends early exactly when its current node has no successors.  A start outside [0, num_nodes) gives a row
+ *     of -1.  Successor ids are not range-checked (the graph build checks them).
+ *   - Every draw is Philox4x32-10(counter = (i lo32, i hi32, step, trial), key = (seed lo32, seed hi32)): the walks
+ *     are a pure function of (graph, nodes, seed).  A uniform slot of a row of deg slots is mulhi64(r64, deg) with
+ *     r64 = (word1 << 32) | word0.
+ *   - random_walk: at most max_depth nodes (max_depth - 1 steps), L = max_depth; each step takes the uniform slot of
+ *     trial 0.
+ *   - node2vec: up to max_depth steps, L = max_depth + 1 (the reference's count).  A step from cur with previous node
+ *     prev takes slot s with probability proportional to w = 1/p if cols[s] == prev, 1 if cols[s] is a successor of
+ *     prev (plus != 0: of any earlier node of the walk), 1/q otherwise; the first step (no prev) is the uniform slot of
+ *     trial 0.  Rejection sampling: trial k proposes the uniform slot of trial k and accepts it iff
+ *     word2 < floor(w / max(1/p, 1, 1/q) * 2^32); after cap = max(16, deg) rejected trials the step is an exact
+ *     float64 inverse CDF over the row in slot order, with u = (r64 of trial cap >> 11) * 2^-53.  Membership is a binary search in
+ *     sorted_cols: the successor columns with every row ascending by id (same indptr).  Cost per trial:
+ *     O(log deg(prev)); plus: O(t log d) at step t.  stats (device, 2 uint64, may be NULL; the caller zeroes it)
+ *     accumulates {candidate draws, fallback steps}.
+ *   - max_depth outside [1, 2^31 - 1), p or q not positive and finite (or with an infinite reciprocal), a negative
+ *     size or a NULL pointer with n > 0: PGLB_EINVAL before any CUDA call. */
+int pglb_random_walk(const int64_t *indptr, const int64_t *cols, int64_t num_nodes, const int64_t *nodes, int64_t n,
+                     int64_t max_depth, uint64_t seed, int64_t *out, void *stream);
+int pglb_node2vec_walk(const int64_t *indptr, const int64_t *cols, const int64_t *sorted_cols, int64_t num_nodes,
+                       const int64_t *nodes, int64_t n, int64_t max_depth, double p, double q, int plus,
+                       uint64_t seed, int64_t *out, uint64_t *stats, void *stream);
+/* The same walks on the host over host arrays, by the kernels' own step function, blocking: mode 0 = random_walk,
+ * 1 = node2vec, 2 = node2vec_plus (p, q and sorted_cols are ignored in mode 0).  stats (host, may be NULL) receives
+ * {candidate draws, fallback steps}.  For tests and small graphs. */
+int pglb_walk_host(const int64_t *indptr, const int64_t *cols, const int64_t *sorted_cols, int64_t num_nodes,
+                   const int64_t *nodes, int64_t n, int64_t max_depth, double p, double q, int mode, uint64_t seed,
+                   int64_t *out, uint64_t *stats);
+
 /* Same contract as pglb_memcpy2d_async, but the copy is done by a kernel through the unified address
  * space (zero-copy loads / stores across PCIe; the host side must be pinned memory).  For narrow column
  * blocks, where the copy engine's 2-D transfers run at about half the PCIe rate.  width, pitches and both

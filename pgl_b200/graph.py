@@ -140,7 +140,7 @@ class Graph(object):
                 if isinstance(ng, np.ndarray):
                     self._num_graph = int(ng.reshape(-1)[0])
             self._nodes = None
-            for a in ("_dst_uniq_ind", "_dst_segment_ids", "_src_uniq_ind", "_src_segment_ids"):
+            for a in ("_dst_uniq_ind", "_dst_segment_ids", "_src_uniq_ind", "_src_segment_ids", "_walk_dev"):
                 self.__dict__.pop(a, None)
             return self
         num_nodes = new["_num_nodes"] if to_t else int(self._n)
@@ -566,6 +566,26 @@ class Graph(object):
             self._adj_dst_index = EdgeIndex.from_edges(
                 u=self._edges[:, 1], v=self._edges[:, 0], num_nodes=self._num_nodes, v_bound=self._n)
         return self._adj_dst_index
+
+    def _walk_csr(self, row_sorted=False):
+        """(indptr, cols, sorted_cols) of the walk kernels (sampling/walk.py) on the device: the src-keyed CSR, and
+        with ``row_sorted`` its columns with every row ascending by id (else None).  That copy is the stable
+        ``csr_build`` of the edges in dst order, built once.  A numpy-mode graph keeps its device copies here (per
+        device), so repeated walks upload the graph once; ``_switch`` drops them."""
+        if self._is_tensor:
+            dev = self._edges.device
+        else:
+            if not torch.cuda.is_available():
+                raise RuntimeError("pgl_b200: random walks run on a CUDA device; none is available")
+            dev = torch.device("cuda", torch.cuda.current_device())
+        cache = self.__dict__.setdefault("_walk_dev", {}).setdefault(str(dev), {})
+        if "indptr" not in cache:
+            src = self.adj_src_index
+            cache["indptr"], cache["cols"] = to_tensor(src._indptr, dev), to_tensor(src._sorted_v, dev)
+        if row_sorted and "sorted" not in cache:
+            dst = self.adj_dst_index
+            cache["sorted"] = ops.csr_build(to_tensor(dst._sorted_v, dev), to_tensor(dst._sorted_u, dev), self._n)[1]
+        return cache["indptr"], cache["cols"], cache.get("sorted") if row_sorted else None
 
     def node_batch_iter(self, batch_size, shuffle=True):
         """reference graph.py:1369-1395."""

@@ -165,6 +165,41 @@ def csr_build(u, v, num_nodes):
     return degree, sv, su, se, indptr
 
 
+# random walks (csrc/walk.cu)
+# ------------------------------------------------------------------------------------------
+
+
+def _walk_args(indptr, cols, nodes):
+    require_cuda(indptr, cols, nodes)
+    nodes = _i64(nodes).reshape(-1).contiguous()
+    # a graph without edges has an empty cols tensor (no address); the kernels never read it then
+    cols_p = _ptr(cols) if cols.numel() else _ptr(indptr)
+    return nodes, cols_p
+
+
+def random_walk(indptr, cols, num_nodes, nodes, max_depth, seed):
+    """pglb_random_walk: [len(nodes), max_depth] int64 walks over the src-keyed CSR (indptr, cols), -1 after a walk
+    ends."""
+    nodes, cols_p = _walk_args(indptr, cols, nodes)
+    out = torch.empty((nodes.numel(), int(max_depth)), dtype=torch.int64, device=nodes.device)
+    with torch.cuda.device(nodes.device):
+        check(lib.pglb_random_walk(_ptr(indptr), cols_p, int(num_nodes), _ptr(nodes), nodes.numel(), int(max_depth),
+                                   int(seed), _ptr(out), _stream()))
+    return out
+
+
+def node2vec_walk(indptr, cols, sorted_cols, num_nodes, nodes, max_depth, p, q, plus, seed, stats=None):
+    """pglb_node2vec_walk: [len(nodes), max_depth + 1] int64 walks, -1 after a walk ends.  sorted_cols: cols with every
+    row ascending by id.  stats: optional int64 CUDA tensor of 2, incremented by (candidate draws, fallback steps)."""
+    nodes, cols_p = _walk_args(indptr, cols, nodes)
+    out = torch.empty((nodes.numel(), int(max_depth) + 1), dtype=torch.int64, device=nodes.device)
+    with torch.cuda.device(nodes.device):
+        check(lib.pglb_node2vec_walk(_ptr(indptr), cols_p, _ptr(sorted_cols) if sorted_cols.numel() else cols_p,
+                                     int(num_nodes), _ptr(nodes), nodes.numel(), int(max_depth), float(p), float(q),
+                                     int(bool(plus)), int(seed), _ptr(out), _ptr(stats), _stream()))
+    return out
+
+
 # partition -> local graph (csrc/localgraph.cu)
 # ------------------------------------------------------------------------------------------
 
