@@ -470,6 +470,62 @@ int pglb_walk_host(const int64_t *indptr, const int64_t *cols, const int64_t *so
                    const int64_t *nodes, int64_t n, int64_t max_depth, double p, double q, int mode, uint64_t seed,
                    int64_t *out, uint64_t *stats);
 
+/* ------------------------------------------------------------------------------------
+ * Graph-level readouts (csrc/readout.cu).  Every entry is keyed by a segment CSR indptr[B + 1] (device int64,
+ * non-decreasing, indptr[0] = 0, indptr[B] = N): segment g is the contiguous rows indptr[g] .. indptr[g + 1] - 1 (a
+ * batched graph's _graph_node_index).  Every output element has exactly one writer, there are no atomics, and the
+ * results are the same from run to run.  Bad arguments return PGLB_EINVAL before any CUDA call.
+ *
+ * Fused attention readout (GlobalAttention, Set2Set; reference pgl/nn/pool.py:121-179):
+ *   out[g] = sum_{i in g} softmax_g(s)_i * x_i,  lse[g] = log sum_{i in g} exp(s_i)
+ * with s_i = gate[i] (gate, [N]) or s_i = <x_i, query[g]> (query, [B, D]); pass exactly one of the two.  x [N, D], out
+ * [B, D] row-major float32, 1 <= D <= 16384.  One pass over x with an online max and sum.  An empty segment gives a
+ * zero row and lse = -inf.  Segments are split into chunks of 2048 rows (boundaries depend on the segment's length
+ * only, so a segment's output is bit-identical wherever it sits in the batch); a longer segment's chunks write
+ * partials to the workspace that a second launch merges in chunk order.  max_len: the longest segment.  With
+ * max_len <= 2048 no workspace is needed (pglb_attn_readout_ws gives 0) and the call is one launch.  A max_len below
+ * the true longest segment still gives correct results, but such a segment is then read as one chunk.
+ * Backward (one launch when max_len <= 2048; a second merges grad_query otherwise): with a_i = exp(s_i - lse_g),
+ *   ds_i = a_i (<x_i, grad_out_g> - <out_g, grad_out_g>),  grad_x_i = a_i grad_out_g (+ ds_i query_g),
+ *   grad_gate_i = ds_i (gate given; grad_gate may be NULL),  grad_query_g = sum_i ds_i x_i (query given). */
+int pglb_attn_readout_ws(int64_t num_segments, int64_t num_rows, int64_t dim, int64_t max_len, size_t *ws_bytes);
+int pglb_attn_readout_f32(const float *x, int64_t num_rows, int64_t dim, const int64_t *indptr, int64_t num_segments,
+                          int64_t max_len, const float *gate, const float *query, float *out, float *lse, void *ws,
+                          size_t ws_bytes, void *stream);
+int pglb_attn_readout_bwd_f32(const float *x, int64_t num_rows, int64_t dim, const int64_t *indptr,
+                              int64_t num_segments, int64_t max_len, const float *gate, const float *query,
+                              const float *out, const float *lse, const float *grad_out, float *grad_x,
+                              float *grad_gate, float *grad_query, void *ws, size_t ws_bytes, void *stream);
+
+/* Segmented top-k (segment_topk / SAGPool; reference pgl/math.py:299-364), two calls:
+ *   count: k_g = min(k, n_g) when k > 0, else ceilf(ratio * (float)n_g) computed in fp32 as the reference does
+ *          (ratio in (0, 1], otherwise PGLB_EINVAL); offsets[0 .. B] (device int64, B + 1) = exclusive prefix of k_g;
+ *          info (device int64[2]) = {offsets[B] (total kept), longest segment}.  One launch.
+ *   fill : perm[offsets[g] + r] = the node of rank r of segment g, r < k_g.  Ranks follow a total order: score
+ *          descending, -0.0 == +0.0, NaN after every number, ties by ascending node index.  max_len = info[1]:
+ *          segments of at most 2048 nodes are ranked in shared memory (one CTA per segment, one launch, no
+ *          workspace); a longer max_len sorts (segment, score) keys with the stable radix sort of pglb_csr_build and
+ *          needs pglb_segment_topk_ws bytes.  Both paths give the same perm.  A max_len below the longest segment
+ *          still gives the same perm: a segment longer than the shared array is then ranked from global memory
+ *          (quadratic in its length). */
+int pglb_segment_topk_count(const int64_t *indptr, int64_t num_segments, float ratio, int64_t k, int64_t *offsets,
+                            int64_t *info, void *stream);
+int pglb_segment_topk_ws(int64_t num_segments, int64_t num_rows, int64_t max_len, size_t *ws_bytes);
+int pglb_segment_topk_fill(const float *scores, int64_t num_rows, const int64_t *indptr, int64_t num_segments,
+                           const int64_t *offsets, int64_t max_len, int64_t *perm, void *ws, size_t ws_bytes,
+                           void *stream);
+
+/* Dense batching (to_dense_batch / segment_padding; reference pgl/utils/transform.py:101-135, pgl/math.py:227-272),
+ * copies by element size (2, 4 or 8 bytes), so exact in every dtype.  Rows are D contiguous elements.
+ *   pad  : out[b, p] (out [B, max_len, D]) = x[indptr[b] + p] for p < n_b, else D copies of the element whose bits are
+ *          the low elem_size bytes of fill_bits.  Each output row is written once; rows of a segment beyond max_len
+ *          are dropped (the caller passes max_len >= the longest segment).
+ *   unpad: out[i] = padded[b, i - indptr[b]] for every row i (the adjoint gather; zeros where i - indptr[b] >= max_len). */
+int pglb_segment_pad(const void *x, int64_t num_rows, int64_t dim, int elem_size, const int64_t *indptr,
+                     int64_t num_segments, int64_t max_len, uint64_t fill_bits, void *out, void *stream);
+int pglb_segment_unpad(const void *padded, int64_t num_segments, int64_t max_len, int64_t dim, int elem_size,
+                       const int64_t *indptr, int64_t num_rows, void *out, void *stream);
+
 /* Same contract as pglb_memcpy2d_async, but the copy is done by a kernel through the unified address
  * space (zero-copy loads / stores across PCIe; the host side must be pinned memory).  For narrow column
  * blocks, where the copy engine's 2-D transfers run at about half the PCIe rate.  width, pitches and both

@@ -75,6 +75,13 @@ inline cudaError_t ensure_dyn_smem(K kernel, int bytes, std::atomic<unsigned lon
 size_t scan_i64_ws_bytes(int64_t n);
 int scan_i64(const int64_t *in, int64_t *out, int64_t n, int inclusive, void *tmp, cudaStream_t stream);
 
+// the stable LSD radix sort of pglb_csr_build (csr_build.cu) over (uint64 key, uint64 value) pairs, key bits [0, bits):
+// equal keys keep their input order.  keys_alt / vals_alt are n-element scratch; *result_in_alt says which pair of
+// buffers holds the sorted result.  tmp: radix_sort_u64_ws_bytes(n) bytes, 256-byte aligned.
+size_t radix_sort_u64_ws_bytes(int64_t n);
+int radix_sort_u64(uint64_t *keys, uint64_t *vals, uint64_t *keys_alt, uint64_t *vals_alt, int64_t n, int bits,
+                   void *tmp, cudaStream_t stream, int *result_in_alt);
+
 // ---- device helpers -------------------------------------------------------------------
 
 // streaming (evict-first) loads for index data that is read exactly once

@@ -298,6 +298,46 @@ struct SortPlan {
     int64_t nb;
 };
 
+// The stable LSD pass loop over key bits [0, bits): one histogram, one scan of the digit-major table and one scatter
+// per 8-bit digit, ping-ponging between (ka, va) and (kb, vb).  On return ka / va name the buffers holding the result.
+// table: 256 * nb int64 with nb = ceil(n / SortGeo<KeyT>::kTile); scan_tmp: scan_ws_bytes(256 * nb).
+template <typename KeyT, typename ValT>
+static int sort_passes(KeyT *&ka, ValT *&va, KeyT *&kb, ValT *&vb, int64_t n, int64_t nb, int bits, int64_t *table,
+                       void *scan_tmp, cudaStream_t stream) {
+    constexpr int IPW = SortGeo<KeyT>::kIpw;
+    for (int shift = 0; shift < bits; shift += 8) {
+        rs_hist_kernel<KeyT, IPW><<<(unsigned)nb, 256, 0, stream>>>(ka, n, shift, nb, table);
+        PGLB_LAUNCH_CHECK("rs_hist_kernel");
+        const int rc = scan_i64(table, table, 256 * nb, /*inclusive=*/0, scan_tmp, stream);
+        if (rc) return rc;
+        rs_scatter_kernel<KeyT, ValT, IPW><<<(unsigned)nb, 256, 0, stream>>>(ka, va, kb, vb, n, shift, nb, table);
+        PGLB_LAUNCH_CHECK("rs_scatter_kernel");
+        std::swap(ka, kb);
+        std::swap(va, vb);
+    }
+    return PGLB_OK;
+}
+
+static int64_t sort_blocks_u64(int64_t n) { return (n + SortGeo<uint64_t>::kTile - 1) / SortGeo<uint64_t>::kTile; }
+
+size_t radix_sort_u64_ws_bytes(int64_t n) {
+    const int64_t nb = std::max<int64_t>(sort_blocks_u64(n), 1);
+    return align_up(sizeof(int64_t) * 256 * (size_t)nb, 256) + scan_ws_bytes(256 * nb);
+}
+
+int radix_sort_u64(uint64_t *keys, uint64_t *vals, uint64_t *keys_alt, uint64_t *vals_alt, int64_t n, int bits,
+                   void *tmp, cudaStream_t stream, int *result_in_alt) {
+    *result_in_alt = 0;
+    if (n <= 0) return PGLB_OK;
+    const int64_t nb = sort_blocks_u64(n);
+    int64_t *table = reinterpret_cast<int64_t *>(tmp);
+    void *scan_tmp = reinterpret_cast<char *>(tmp) + align_up(sizeof(int64_t) * 256 * (size_t)nb, 256);
+    uint64_t *ka = keys, *va = vals, *kb = keys_alt, *vb = vals_alt;
+    const int rc = sort_passes<uint64_t, uint64_t>(ka, va, kb, vb, n, nb, bits, table, scan_tmp, stream);
+    *result_in_alt = ka != keys;
+    return rc;
+}
+
 template <typename KeyT, typename ValT>
 static SortPlan plan(int64_t E, int64_t N) {
     SortPlan pl;
@@ -357,19 +397,8 @@ static int run(const int64_t *u, int64_t us, const int64_t *v, int64_t vs, int64
         if (rc) return rc;
     }
     if (E > 0) {
-        constexpr int IPW = SortGeo<KeyT>::kIpw;
-        const int bits = key_bits(N);
-        for (int shift = 0; shift < bits; shift += 8) {
-            rs_hist_kernel<KeyT, IPW><<<(unsigned)pl.nb, 256, 0, stream>>>(ka, E, shift, pl.nb, table);
-            PGLB_LAUNCH_CHECK("rs_hist_kernel");
-            const int rc = scan_i64(table, table, 256 * pl.nb, /*inclusive=*/0, scan_tmp, stream);
-            if (rc) return rc;
-            rs_scatter_kernel<KeyT, ValT, IPW><<<(unsigned)pl.nb, 256, 0, stream>>>(ka, va, kb, vb, E, shift,
-                                                                                  pl.nb, table);
-            PGLB_LAUNCH_CHECK("rs_scatter_kernel");
-            std::swap(ka, kb);
-            std::swap(va, vb);
-        }
+        const int rc = sort_passes<KeyT, ValT>(ka, va, kb, vb, E, pl.nb, key_bits(N), table, scan_tmp, stream);
+        if (rc) return rc;
         emit_sorted_kernel<KeyT, ValT><<<blocks, 256, 0, stream>>>(ka, va, v, vs, E, su, sv, se);
         PGLB_LAUNCH_CHECK("emit_sorted_kernel");
     }

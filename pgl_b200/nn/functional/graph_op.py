@@ -1,9 +1,11 @@
 """Graph functional ops on the send/recv path (mirror of reference
-pgl/nn/functional/graph_op.py:29-55,101-123)."""
+pgl/nn/functional/graph_op.py:29-123)."""
 
 from ... import math, ops
 
-__all__ = ["degree_norm", "graph_pool", "edge_softmax"]
+import torch
+
+__all__ = ["degree_norm", "graph_pool", "graph_norm", "edge_softmax"]
 
 
 def degree_norm(graph, mode="indegree"):
@@ -25,6 +27,19 @@ def degree_norm(graph, mode="indegree"):
 def graph_pool(graph, feature, pool_type):
     """reference graph_op.py:58-76: segment pool over graph_node_id."""
     return math.segment_pool(feature, graph.graph_node_id, pool_type)
+
+
+def graph_norm(graph, feature):
+    """reference graph_op.py:78-98: every node's feature divided by sqrt(number of nodes of its graph), in the
+    reference's op order (segment_sum of ones, sqrt, gather, divide) so the result is the same bit for bit.  A
+    bfloat16 / float16 feature is divided in fp32 and rounded once back to its own dtype."""
+    nodes = torch.ones((graph._n, 1), dtype=torch.float32, device=feature.device)
+    norm = graph_pool(graph, nodes, pool_type="sum")
+    norm = torch.sqrt(norm)
+    norm = ops.gather_rows(norm, graph.graph_node_id)
+    if feature.dtype in ops.HALF_DTYPES:
+        return (feature.float() / norm).to(feature.dtype)
+    return feature / norm
 
 
 def edge_softmax(graph, logits, norm_by="dst"):

@@ -200,6 +200,220 @@ def node2vec_walk(indptr, cols, sorted_cols, num_nodes, nodes, max_depth, p, q, 
     return out
 
 
+# graph-level readouts (csrc/readout.cu)
+# ------------------------------------------------------------------------------------------
+
+
+def segment_max_len(indptr):
+    """Longest segment of a segment CSR: one 8-byte read back, cached on the indptr tensor so repeated readouts over
+    the same batch (Set2Set's iterations) read it once.  The value only picks the kernels' work layout: a stale one
+    (an indptr refilled in place) still gives correct results (DESIGN section 4.10)."""
+    cached = getattr(indptr, "_pglb_max_len", None)
+    if cached is None:
+        B = int(indptr.numel()) - 1
+        cached = int((indptr[1:] - indptr[:-1]).max().item()) if B > 0 else 0
+        indptr._pglb_max_len = cached
+    return cached
+
+
+def _readout_ws(B, N, D, max_len, dev):
+    need = ctypes.c_size_t(0)
+    check(lib.pglb_attn_readout_ws(B, N, D, max_len, ctypes.byref(need)))
+    return workspace(dev, need.value) if need.value else None
+
+
+def _attn_readout_raw(x2, indptr, gate, query, max_len):
+    N, D = int(x2.shape[0]), int(x2.shape[1])
+    B = int(indptr.numel()) - 1
+    out = torch.empty((B, D), dtype=torch.float32, device=x2.device)
+    lse = torch.empty(B, dtype=torch.float32, device=x2.device)
+    ws = _readout_ws(B, N, D, max_len, x2.device)
+    with torch.cuda.device(x2.device):
+        check(lib.pglb_attn_readout_f32(_ptr(x2), N, D, _ptr(indptr), B, max_len, _ptr(gate), _ptr(query), _ptr(out),
+                                        _ptr(lse), _ptr(ws), ws.numel() if ws is not None else 0, _stream()))
+    return out, lse
+
+
+class _AttnReadout(torch.autograd.Function):
+    """Fused attention readout; saves lse and the output r for the one-launch backward."""
+
+    @staticmethod
+    def forward(ctx, x2, gate, query, indptr, max_len):
+        out, lse = _attn_readout_raw(x2, indptr, gate, query, max_len)
+        ctx.meta = (indptr, max_len)
+        ctx.save_for_backward(x2, gate, query, out, lse)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        indptr, max_len = ctx.meta
+        x2, gate, query, out, lse = ctx.saved_tensors
+        g = g.contiguous()
+        N, D = int(x2.shape[0]), int(x2.shape[1])
+        B = int(indptr.numel()) - 1
+        gx = torch.empty_like(x2)
+        gg = torch.empty_like(gate) if gate is not None else None
+        gq = torch.empty_like(query) if query is not None else None
+        ws = _readout_ws(B, N, D, max_len, x2.device)
+        with torch.cuda.device(x2.device):
+            check(lib.pglb_attn_readout_bwd_f32(_ptr(x2), N, D, _ptr(indptr), B, max_len, _ptr(gate), _ptr(query),
+                                                _ptr(out), _ptr(lse), _ptr(g), _ptr(gx), _ptr(gg), _ptr(gq), _ptr(ws),
+                                                ws.numel() if ws is not None else 0, _stream()))
+        return gx, gg, gq, None, None
+
+
+@f64_through
+def attn_readout(x, indptr, gate=None, query=None, return_lse=False):
+    """out[g] = sum_{i in g} softmax_g(s)_i * x_i over the segments of indptr (int64 [B + 1]), with s = gate ([N] or
+    [N, 1]: GlobalAttention) or s_i = <x_i, query[g]> (query [B, D]: Set2Set) -- the reference's gather, multiply,
+    reduce, 7-op segment_softmax, multiply and segment_sum (pgl/nn/pool.py:139-142, 177-178) in one pass over x.
+    Gradients reach x, gate and query."""
+    if (gate is None) == (query is None):
+        raise ValueError("attn_readout: pass exactly one of gate and query")
+    require_cuda(x, indptr, gate, query)
+    x2 = _f32_2d(x)
+    if x.dim() != 2:
+        raise ValueError("attn_readout: x must be [N, D]")
+    indptr = _i64(indptr).contiguous()
+    B, N, D = int(indptr.numel()) - 1, int(x2.shape[0]), int(x2.shape[1])
+    if gate is not None:
+        if gate.numel() != N:
+            raise ValueError("attn_readout: gate must hold one score per row of x")
+        gate = _f32_2d(gate.reshape(N, 1)).reshape(N)
+    else:
+        if tuple(query.shape) != (B, D):
+            raise ValueError("attn_readout: query must be [num_segments, D]")
+        query = _f32_2d(query)
+    max_len = segment_max_len(indptr)
+    grad = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x2, gate, query))
+    if grad and not return_lse:
+        return _AttnReadout.apply(x2, gate, query, indptr, max_len)
+    out, lse = _attn_readout_raw(x2, indptr, gate, query, max_len)
+    return (out, lse) if return_lse else out
+
+
+def segment_topk_perm(scores, indptr, ratio):
+    """perm of segment_topk (reference pgl/math.py:342-359): for every segment g of indptr, the nodes of its first
+    k_g ranks (score descending, -0.0 == +0.0, NaN last, ties by ascending node index), segments in order.
+    k_g = ceil(fp32(ratio) * fp32(n_g)) for a float ratio in (0, 1], min(ratio, n_g) for an int ratio >= 1.  Scores
+    are ranked in float32, as the reference's dense score matrix holds them.  One 16-byte read back (the total and the
+    longest segment), as the reference also synchronises here."""
+    if isinstance(ratio, int):
+        if ratio < 1:
+            raise ValueError("segment_topk: an int ratio must be at least 1, got %d" % ratio)
+        k, r = int(ratio), 0.0
+    else:
+        r = float(ratio)
+        if not 0.0 < r <= 1.0:
+            raise ValueError("segment_topk: a float ratio must lie in (0, 1], got %r" % ratio)
+        k = 0
+    require_cuda(scores, indptr)
+    s = scores.reshape(-1).to(torch.float32).contiguous()
+    indptr = _i64(indptr).contiguous()
+    B, N = int(indptr.numel()) - 1, int(s.numel())
+    dev = s.device
+    offsets = torch.empty(B + 1, dtype=torch.int64, device=dev)
+    info = torch.empty(2, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        check(lib.pglb_segment_topk_count(_ptr(indptr), B, r, k, _ptr(offsets), _ptr(info), _stream()))
+        total, max_len = (int(v) for v in info.tolist())
+        perm = torch.empty(total, dtype=torch.int64, device=dev)
+        need = ctypes.c_size_t(0)
+        check(lib.pglb_segment_topk_ws(B, N, max_len, ctypes.byref(need)))
+        ws = workspace(dev, need.value) if need.value else None
+        check(lib.pglb_segment_topk_fill(_ptr(s), N, _ptr(indptr), B, _ptr(offsets), max_len, _ptr(perm), _ptr(ws),
+                                         ws.numel() if ws is not None else 0, _stream()))
+    return perm
+
+
+_BITS_VIEW = {2: torch.int16, 4: torch.int32, 8: torch.int64}
+
+
+def _fill_bits(value, dtype):
+    t = torch.tensor([value], dtype=dtype)
+    size = t.element_size()
+    return int(t.view(_BITS_VIEW[size]).item()) & ((1 << (8 * size)) - 1)
+
+
+def _rows_of(t):
+    if t.element_size() not in _BITS_VIEW:
+        raise TypeError("pgl_b200: segment padding copies elements of 2, 4 or 8 bytes, got %s" % t.dtype)
+    t2 = t.reshape(t.shape[0], -1) if t.dim() != 2 else t
+    return t2.contiguous()
+
+
+def _segment_pad_raw(x2, indptr, max_len, fill_bits):
+    N, D = int(x2.shape[0]), int(x2.shape[1])
+    B = int(indptr.numel()) - 1
+    out = torch.empty((B, max_len, D), dtype=x2.dtype, device=x2.device)
+    with torch.cuda.device(x2.device):
+        check(lib.pglb_segment_pad(_ptr(x2), N, D, x2.element_size(), _ptr(indptr), B, max_len, fill_bits, _ptr(out),
+                                   _stream()))
+    return out
+
+
+def _segment_unpad_raw(p3, indptr, num_rows):
+    B, L, D = int(p3.shape[0]), int(p3.shape[1]), int(p3.shape[2])
+    out = torch.empty((int(num_rows), D), dtype=p3.dtype, device=p3.device)
+    with torch.cuda.device(p3.device):
+        check(lib.pglb_segment_unpad(_ptr(p3), B, L, D, p3.element_size(), _ptr(indptr), int(num_rows), _ptr(out),
+                                     _stream()))
+    return out
+
+
+class _SegmentPad(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x2, indptr, max_len, fill_bits):
+        ctx.meta = (indptr, int(x2.shape[0]))
+        return _segment_pad_raw(x2, indptr, max_len, fill_bits)
+
+    @staticmethod
+    def backward(ctx, g):
+        indptr, n = ctx.meta
+        return _segment_unpad_raw(g.contiguous(), indptr, n), None, None, None
+
+
+class _SegmentUnpad(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, p3, indptr, num_rows):
+        ctx.meta = (indptr, int(p3.shape[1]))
+        return _segment_unpad_raw(p3, indptr, num_rows)
+
+    @staticmethod
+    def backward(ctx, g):
+        indptr, max_len = ctx.meta
+        return _segment_pad_raw(g.contiguous(), indptr, max_len, 0), None, None
+
+
+def segment_pad(x, indptr, max_len, fill_value=0):
+    """[N, *F] -> [B, max_len, *F]: row p of block b is x[indptr[b] + p] for p < n_b, else fill_value.  Native in
+    every dtype of 2, 4 or 8 bytes (a copy, so exact); max_len must be at least the longest segment.  The gradient is
+    segment_unpad."""
+    require_cuda(x, indptr)
+    indptr = _i64(indptr).contiguous()
+    x2 = _rows_of(x)
+    bits = _fill_bits(fill_value, x2.dtype)
+    if x2.requires_grad and torch.is_grad_enabled():
+        out = _SegmentPad.apply(x2, indptr, int(max_len), bits)
+    else:
+        out = _segment_pad_raw(x2, indptr, int(max_len), bits)
+    return out.reshape(out.shape[:2] + tuple(x.shape[1:]))
+
+
+def segment_unpad(padded, indptr, num_rows):
+    """The adjoint gather of segment_pad: [B, max_len, *F] -> [num_rows, *F], row i = padded[b, i - indptr[b]]."""
+    require_cuda(padded, indptr)
+    indptr = _i64(indptr).contiguous()
+    if padded.element_size() not in _BITS_VIEW:
+        raise TypeError("pgl_b200: segment padding copies elements of 2, 4 or 8 bytes, got %s" % padded.dtype)
+    p3 = padded.reshape(padded.shape[0], padded.shape[1], -1).contiguous()
+    if p3.requires_grad and torch.is_grad_enabled():
+        out = _SegmentUnpad.apply(p3, indptr, int(num_rows))
+    else:
+        out = _segment_unpad_raw(p3, indptr, int(num_rows))
+    return out.reshape((int(num_rows),) + tuple(padded.shape[2:]))
+
+
 # partition -> local graph (csrc/localgraph.cu)
 # ------------------------------------------------------------------------------------------
 

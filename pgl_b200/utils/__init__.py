@@ -1,1 +1,1 @@
-from . import helper, op, edge_index, relabel  # noqa: F401
+from . import helper, op, edge_index, relabel, transform  # noqa: F401
