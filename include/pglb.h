@@ -397,6 +397,73 @@ int pglb_gat_bwd_edge_drop_x16(const int64_t *rows, const int64_t *cols, const i
 int pglb_attn_dropout_keep_host(uint64_t seed, uint64_t offset, float attn_drop, int64_t slot0, int64_t n_slots,
                                 int64_t H, uint32_t *keep_words);
 
+/* Dot-product attention of TransformerConv without edge features (pgl/nn/conv.py:808-847: send q[dst] * k[src] summed
+ * over the head dim, softmax over the in-edges, weighted sum of v[src]) in ONE pass, the GAT kernel's online softmax:
+ *   s_j = <q[d,h,:], k[cols[j],h,:]>,  lse[d,h] = log sum_j exp(s_j),  out[d,h,:] = sum_j exp(s_j - lse) v[cols[j],h,:]
+ * over the dst-CSR slots j of row d (rows without in-edges: out = 0).  q is already scaled by 1 / sqrt(head_dim).  No
+ * [E, H * head_dim] product and no [E, H] score is ever written.
+ *   - q [n_dst, H * head_dim], k and v [n_src, H * head_dim], out [n_dst, ...] with row strides ldq, ldk, ldv, ldo in
+ *     elements.  lse [n_dst, H] float32 is nullable (inference); when given, rows with at least one in-edge are
+ *     written (others are not) -- all the edge backward needs.  ws as pglb_spmm_csr_ws(D = H * head_dim).
+ *   - Shapes: D = H * head_dim <= 128 in 16-byte rows (D % 4 == 0 float32, D % 8 == 0 16-bit), head_dim in
+ *     {4, 8, ..., 128}, n_src < 2^31 - 1: otherwise PGLB_EUNSUPPORTED.  q, k, v, out not 16-byte aligned, a row stride
+ *     below D or not a multiple of 16 bytes: PGLB_ESHAPE.
+ *   - _x16 (`dtype` bfloat16 / float16 q, k, v and out; lse float32): rows are widened exactly and every later operation
+ *     is the float32 kernel's in the same slot order, rounded once on the store, so out == round16(pglb_dot_attn_csr_f32
+ *     on the widened q, k, v) and lse equals its lse, bit for bit.  Unknown dtype: PGLB_EINVAL.
+ *   - _drop_ (attention dropout): the arguments plus attn_drop, seed, offset, the stream and rules of the GAT dropout
+ *     entries above (same keep word per dst-CSR slot and head, H % 4 == 0):
+ *     out = sum_j s m_j exp(s_j - lse) v[cols[j]], and lse is bitwise the value without dropout.
+ *   - All argument checks precede any CUDA call. */
+int pglb_dot_attn_csr_f32(const int64_t *indptr, const int64_t *cols, const float *q, int64_t ldq, const float *k,
+                          int64_t ldk, const float *v, int64_t ldv, float *out, int64_t ldo, float *lse, int64_t n_dst,
+                          int64_t n_src, int64_t num_edges, int64_t H, int64_t head_dim, void *ws, size_t ws_bytes,
+                          void *stream);
+int pglb_dot_attn_csr_x16(const int64_t *indptr, const int64_t *cols, const void *q, int64_t ldq, const void *k,
+                          int64_t ldk, const void *v, int64_t ldv, void *out, int64_t ldo, float *lse, int64_t n_dst,
+                          int64_t n_src, int64_t num_edges, int64_t H, int64_t head_dim, int dtype, void *ws,
+                          size_t ws_bytes, void *stream);
+int pglb_dot_attn_drop_csr_f32(const int64_t *indptr, const int64_t *cols, const float *q, int64_t ldq, const float *k,
+                               int64_t ldk, const float *v, int64_t ldv, float *out, int64_t ldo, float *lse,
+                               int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H, int64_t head_dim,
+                               float attn_drop, uint64_t seed, uint64_t offset, void *ws, size_t ws_bytes, void *stream);
+int pglb_dot_attn_drop_csr_x16(const int64_t *indptr, const int64_t *cols, const void *q, int64_t ldq, const void *k,
+                               int64_t ldk, const void *v, int64_t ldv, void *out, int64_t ldo, float *lse,
+                               int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H, int64_t head_dim, int dtype,
+                               float attn_drop, uint64_t seed, uint64_t offset, void *ws, size_t ws_bytes, void *stream);
+
+/* Per-edge part of that attention's backward.  rows / cols / eid as pglb_gat_bwd_edge_f32; lse from the forward;
+ * grad_out = G.  With s and a = exp(s - lse[dst,h]) rebuilt (s bit for bit the forward's score):
+ *   beta_e[e,h] = a,   ds_e[e,h] = a * (<G[dst,h,:], v[src,h,:]> - <G[dst,h,:], out[dst,h,:]>)
+ * both [num_edges, H] float32 in ORIGINAL edge order.  The caller finishes with three aggregations:
+ * grad q = send_ue_recv(k, ds_e, mul, sum) over the dst-keyed CSR, grad k = send_ue_recv(q, ds_e, mul, sum) and
+ * grad v = send_ue_recv(grad_out, beta_e, mul, sum) over the src-keyed CSR.  head_dim in {4, 8, ..., 128},
+ * H*head_dim <= 128, rows 16-byte aligned.
+ *   - _x16: the row inputs in `dtype`, widened exactly; beta_e and ds_e equal the f32 entry's on the widened inputs
+ *     bit for bit.
+ *   - _drop_: the forward's attn_drop, seed, offset; da is multiplied by s m, and beta_e = m ? fl(a * s) : 0. */
+int pglb_dot_attn_bwd_edge_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *q,
+                               int64_t ldq, const float *k, int64_t ldk, const float *v, int64_t ldv,
+                               const float *grad_out, int64_t ldg, const float *out, int64_t ldo, const float *lse,
+                               int64_t num_edges, int64_t H, int64_t head_dim, float *beta_e, float *ds_e,
+                               void *stream);
+int pglb_dot_attn_bwd_edge_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *q,
+                               int64_t ldq, const void *k, int64_t ldk, const void *v, int64_t ldv,
+                               const void *grad_out, int64_t ldg, const void *out, int64_t ldo, const float *lse,
+                               int64_t num_edges, int64_t H, int64_t head_dim, int dtype, float *beta_e, float *ds_e,
+                               void *stream);
+int pglb_dot_attn_bwd_edge_drop_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *q,
+                                    int64_t ldq, const float *k, int64_t ldk, const float *v, int64_t ldv,
+                                    const float *grad_out, int64_t ldg, const float *out, int64_t ldo,
+                                    const float *lse, int64_t num_edges, int64_t H, int64_t head_dim, float attn_drop,
+                                    uint64_t seed, uint64_t offset, float *beta_e, float *ds_e, void *stream);
+int pglb_dot_attn_bwd_edge_drop_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *q,
+                                    int64_t ldq, const void *k, int64_t ldk, const void *v, int64_t ldv,
+                                    const void *grad_out, int64_t ldg, const void *out, int64_t ldo,
+                                    const float *lse, int64_t num_edges, int64_t H, int64_t head_dim, int dtype,
+                                    float attn_drop, uint64_t seed, uint64_t offset, float *beta_e, float *ds_e,
+                                    void *stream);
+
 /* out[M, N] = act(x[M, K] @ w[K, N] + bias[N]) -- the dense transform of the conv layers
  * (pgl/nn/conv.py:238-251 GCNConv: `self.linear(...)`, `+ self.bias`, activation; the same Linear in
  * GATConv :321 / GraphSageConv :107-108) on the tensor cores with 3xTF32 error compensation (fp32-level

@@ -118,6 +118,22 @@ _SIGS = {
     "pglb_gat_bwd_edge_drop_x16": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _p, _p, ctypes.c_float,
                                            _i64, _i64, _i64, c_int, ctypes.c_float, _u64, _u64, _p, _p, _p]),
     "pglb_attn_dropout_keep_host": (c_int, [_u64, _u64, ctypes.c_float, _i64, _i64, _i64, _p]),
+    "pglb_dot_attn_csr_f32": (c_int, [_p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _i64, _i64, _i64, _i64,
+                                      _p, c_size_t, _p]),
+    "pglb_dot_attn_csr_x16": (c_int, [_p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _i64, _i64, _i64, _i64,
+                                      c_int, _p, c_size_t, _p]),
+    "pglb_dot_attn_drop_csr_f32": (c_int, [_p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _i64, _i64, _i64,
+                                           _i64, ctypes.c_float, _u64, _u64, _p, c_size_t, _p]),
+    "pglb_dot_attn_drop_csr_x16": (c_int, [_p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _i64, _i64, _i64,
+                                           _i64, c_int, ctypes.c_float, _u64, _u64, _p, c_size_t, _p]),
+    "pglb_dot_attn_bwd_edge_f32": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _i64,
+                                           _i64, _p, _p, _p]),
+    "pglb_dot_attn_bwd_edge_x16": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _i64,
+                                           _i64, c_int, _p, _p, _p]),
+    "pglb_dot_attn_bwd_edge_drop_f32": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64,
+                                                _i64, _i64, ctypes.c_float, _u64, _u64, _p, _p, _p]),
+    "pglb_dot_attn_bwd_edge_drop_x16": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64,
+                                                _i64, _i64, c_int, ctypes.c_float, _u64, _u64, _p, _p, _p]),
     "pglb_gat_attention_csr_f32": (c_int, [_p, _p, _p, _p, ctypes.c_float, _p, _i64, _i64, _i64, _p,
                                            c_size_t, _p]),
     "pglb_sddmm_dot_f32": (c_int, [_p, _p, _p, _i64, _p, _i64, _i64, _i64, _i64, _p, _p]),

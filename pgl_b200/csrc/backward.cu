@@ -202,6 +202,87 @@ __global__ void __launch_bounds__(256) gat_bwd_edge_kernel(
     }
 }
 
+// Backward of the single-pass dot-product attention (pglb_dot_attn_*), the per-edge part.  With
+//   s = <q[dst,h,:], k[src,h,:]>,  a = exp(s - lse[dst,h]),  out[dst,h,:] = sum a v[src,h,:],  G = d loss / d out:
+//   da = <G[dst,h,:], v[src,h,:]>,   delta = <G[dst,h,:], out[dst,h,:]>,   ds = a (da - delta)
+// written, with beta = a (the weight grad v is aggregated with), as [E, H] fp32 in ORIGINAL edge order.  The walk is
+// gat_bwd_edge_kernel's: dst-CSR slots, q / G / out / lse re-read only when the row changes, four slots' k and v rows
+// in flight per lane.  s is formed by the forward's dot4_lane + head_sum_lanes, so it is the forward's score bit for bit.
+// T: element type of q, k, v, G and out (16-bit rows are widened exactly; everything after is the fp32 kernel's).
+// DROP: da = s m da and beta = m ? fl(a s) : 0 (m the slot and head's keep bit, s = 1 / (1 - p)); delta is unchanged.
+template <int LPH, typename T, bool DROP>
+__global__ void __launch_bounds__(256) dot_attn_bwd_edge_kernel(
+    const int64_t *__restrict__ rows, const int64_t *__restrict__ cols, const int64_t *__restrict__ eid,
+    const T *__restrict__ q, int64_t ldq, const T *__restrict__ k, int64_t ldk, const T *__restrict__ v, int64_t ldv,
+    const T *__restrict__ g, int64_t ldg, const T *__restrict__ out, int64_t ldo, const float *__restrict__ lse,
+    int64_t E, int H, int D, float *__restrict__ beta_e, float *__restrict__ ds_e, const AttnDrop drop) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const bool act = lane * 4 < D;
+    const int head = act ? lane / LPH : 0;
+    const bool lead = act && (lane % LPH) == 0;
+    for (int64_t base = warp * 32; base < E; base += nwarps * 32) {
+        const int64_t j = base + lane;
+        const bool in = j < E;
+        const long long r_l = in ? ld_stream(rows + j) : 0;
+        const long long c_l = in ? ld_stream(cols + j) : 0;
+        const long long i_l = in ? (eid ? ld_stream(eid + j) : j) : 0;
+        unsigned kw_l = 0;
+        if constexpr (DROP) kw_l = attn_keep_word(drop, (uint64_t)j, H);
+        const int cnt = (E - base) < 32 ? (int)(E - base) : 32;
+        long long cur = -1;
+        float4 q4 = make_float4(0.f, 0.f, 0.f, 0.f), g4 = q4;
+        float ls = 0.f, delta = 0.f;
+        for (int k0 = 0; k0 < cnt; k0 += 4) {
+            float4 kv[4], vv[4];
+            long long rr[4], ii[4];
+            unsigned kk[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const int s = (k0 + u) & 31;
+                const long long cc = __shfl_sync(0xffffffffu, c_l, s);
+                rr[u] = __shfl_sync(0xffffffffu, r_l, s);
+                ii[u] = __shfl_sync(0xffffffffu, i_l, s);
+                if constexpr (DROP) kk[u] = __shfl_sync(0xffffffffu, kw_l, s);
+                kv[u] = vv[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (k0 + u < cnt && act) {
+                    kv[u] = ldg_row4<T>(k + cc * ldk + lane * 4);
+                    vv[u] = ldg_row4<T>(v + cc * ldv + lane * 4);
+                }
+            }
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                if (k0 + u >= cnt) break;
+                if (rr[u] != cur) {  // warp-uniform
+                    cur = rr[u];
+                    float d = 0.f;
+                    if (act) {
+                        q4 = ldg_row4<T>(q + cur * ldq + lane * 4);
+                        g4 = ldg_row4<T>(g + cur * ldg + lane * 4);
+                        d = dot4_lane(g4, ldg_row4<T>(out + cur * ldo + lane * 4));
+                        ls = __ldg(lse + cur * H + head);
+                    }
+                    delta = head_sum_lanes(d, LPH);
+                }
+                const float sc = head_sum_lanes(dot4_lane(q4, kv[u]), LPH);
+                float da = head_sum_lanes(dot4_lane(g4, vv[u]), LPH);
+                const float a = expf(sc - ls);
+                float beta = a;
+                if constexpr (DROP) {
+                    const bool keep = (kk[u] >> head) & 1u;
+                    da = keep ? drop.scale * da : 0.f;
+                    beta = keep ? a * drop.scale : 0.f;
+                }
+                if (lead) {
+                    beta_e[ii[u] * H + head] = beta;
+                    ds_e[ii[u] * H + head] = a * (da - delta);
+                }
+            }
+        }
+    }
+}
+
 static inline int grid_of(int64_t total, int cap_mult) {
     int64_t b = (total + 255) / 256;
     const int64_t cap = (int64_t)sm_count() * cap_mult;
@@ -365,6 +446,115 @@ extern "C" int pglb_gat_bwd_edge_drop_x16(const int64_t *rows, const int64_t *co
                                                  stream_, &drop);
     return gat_bwd_edge_entry<__half>(name, rows, cols, eid, f, ldf, grad_out, ldg, out, ldo, attn_src, attn_dst, lse,
                                       negative_slope, num_edges, H, head_dim, alpha_e, dz_e, stream_, &drop);
+}
+
+// The checks and the launch of the dot-product attention's edge-backward entries (include/pglb.h).  T: element type of
+// q, k, v, grad_out and out, rows 16-byte aligned.  drop (nullable): the attention-dropout stream (H % 4 == 0 then).
+template <typename T>
+static int dot_attn_bwd_edge_entry(const char *name, const int64_t *rows, const int64_t *cols, const int64_t *eid,
+                                   const void *q_, int64_t ldq, const void *k_, int64_t ldk, const void *v_, int64_t ldv,
+                                   const void *g_, int64_t ldg, const void *out_, int64_t ldo, const float *lse,
+                                   int64_t num_edges, int64_t H, int64_t head_dim, float *beta_e, float *ds_e,
+                                   void *stream_, const AttnDrop *drop) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    const T *q = reinterpret_cast<const T *>(q_), *k = reinterpret_cast<const T *>(k_),
+            *v = reinterpret_cast<const T *>(v_), *g = reinterpret_cast<const T *>(g_),
+            *out = reinterpret_cast<const T *>(out_);
+    constexpr int64_t B = sizeof(T);
+    PGLB_CHECK_ARG(num_edges >= 0 && H > 0 && head_dim > 0, PGLB_EINVAL, "%s: bad size", name);
+    const int64_t D = H * head_dim;
+    const int64_t lph = head_dim / 4;
+    PGLB_CHECK_ARG(D <= 128 && head_dim % 4 == 0 && (lph & (lph - 1)) == 0, PGLB_EUNSUPPORTED,
+                   "%s: needs H*head_dim <= 128 and head_dim in {4, 8, 16, 32, 64, 128}", name);
+    PGLB_CHECK_ARG(!drop || H % 4 == 0, PGLB_EUNSUPPORTED, "%s: needs H %% 4 == 0", name);
+    if (num_edges == 0) return PGLB_OK;
+    PGLB_CHECK_ARG(rows && cols && q && k && v && g && out && lse && beta_e && ds_e, PGLB_EINVAL, "%s: NULL pointer",
+                   name);
+    auto a16 = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
+    PGLB_CHECK_ARG(ldq >= D && ldk >= D && ldv >= D && ldg >= D && ldo >= D && (ldq * B) % 16 == 0 &&
+                       (ldk * B) % 16 == 0 && (ldv * B) % 16 == 0 && (ldg * B) % 16 == 0 && (ldo * B) % 16 == 0 &&
+                       a16(q) && a16(k) && a16(v) && a16(g) && a16(out),
+                   PGLB_ESHAPE, "%s: rows must be 16-byte aligned", name);
+    const int grid = grid_of(num_edges, 64);  // a warp per 32 slots, grid-stride
+    const AttnDrop dr = drop ? *drop : AttnDrop{};
+#define PGLB_DBE(L)                                                                                                   \
+    do {                                                                                                              \
+        if (drop)                                                                                                     \
+            dot_attn_bwd_edge_kernel<L, T, true><<<grid, 256, 0, stream>>>(rows, cols, eid, q, ldq, k, ldk, v, ldv,   \
+                                                                           g, ldg, out, ldo, lse, num_edges, (int)H,  \
+                                                                           (int)D, beta_e, ds_e, dr);                 \
+        else                                                                                                          \
+            dot_attn_bwd_edge_kernel<L, T, false><<<grid, 256, 0, stream>>>(rows, cols, eid, q, ldq, k, ldk, v, ldv,  \
+                                                                            g, ldg, out, ldo, lse, num_edges, (int)H, \
+                                                                            (int)D, beta_e, ds_e, dr);                \
+    } while (0)
+    switch ((int)lph) {
+        case 1: PGLB_DBE(1); break;
+        case 2: PGLB_DBE(2); break;
+        case 4: PGLB_DBE(4); break;
+        case 8: PGLB_DBE(8); break;
+        case 16: PGLB_DBE(16); break;
+        default: PGLB_DBE(32); break;
+    }
+#undef PGLB_DBE
+    PGLB_LAUNCH_CHECK("dot_attn_bwd_edge_kernel");
+    return PGLB_OK;
+}
+
+extern "C" int pglb_dot_attn_bwd_edge_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *q,
+                                          int64_t ldq, const float *k, int64_t ldk, const float *v, int64_t ldv,
+                                          const float *grad_out, int64_t ldg, const float *out, int64_t ldo,
+                                          const float *lse, int64_t num_edges, int64_t H, int64_t head_dim,
+                                          float *beta_e, float *ds_e, void *stream_) {
+    return dot_attn_bwd_edge_entry<float>("pglb_dot_attn_bwd_edge_f32", rows, cols, eid, q, ldq, k, ldk, v, ldv,
+                                          grad_out, ldg, out, ldo, lse, num_edges, H, head_dim, beta_e, ds_e, stream_,
+                                          nullptr);
+}
+
+extern "C" int pglb_dot_attn_bwd_edge_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *q,
+                                          int64_t ldq, const void *k, int64_t ldk, const void *v, int64_t ldv,
+                                          const void *grad_out, int64_t ldg, const void *out, int64_t ldo,
+                                          const float *lse, int64_t num_edges, int64_t H, int64_t head_dim, int dtype,
+                                          float *beta_e, float *ds_e, void *stream_) {
+    const char *name = "pglb_dot_attn_bwd_edge_x16";
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    if (dtype == PGLB_DTYPE_BF16)
+        return dot_attn_bwd_edge_entry<__nv_bfloat16>(name, rows, cols, eid, q, ldq, k, ldk, v, ldv, grad_out, ldg, out,
+                                                      ldo, lse, num_edges, H, head_dim, beta_e, ds_e, stream_, nullptr);
+    return dot_attn_bwd_edge_entry<__half>(name, rows, cols, eid, q, ldq, k, ldk, v, ldv, grad_out, ldg, out, ldo, lse,
+                                           num_edges, H, head_dim, beta_e, ds_e, stream_, nullptr);
+}
+
+extern "C" int pglb_dot_attn_bwd_edge_drop_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid,
+                                               const float *q, int64_t ldq, const float *k, int64_t ldk, const float *v,
+                                               int64_t ldv, const float *grad_out, int64_t ldg, const float *out,
+                                               int64_t ldo, const float *lse, int64_t num_edges, int64_t H,
+                                               int64_t head_dim, float attn_drop, uint64_t seed, uint64_t offset,
+                                               float *beta_e, float *ds_e, void *stream_) {
+    const char *name = "pglb_dot_attn_bwd_edge_drop_f32";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    return dot_attn_bwd_edge_entry<float>(name, rows, cols, eid, q, ldq, k, ldk, v, ldv, grad_out, ldg, out, ldo, lse,
+                                          num_edges, H, head_dim, beta_e, ds_e, stream_, &drop);
+}
+
+extern "C" int pglb_dot_attn_bwd_edge_drop_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid,
+                                               const void *q, int64_t ldq, const void *k, int64_t ldk, const void *v,
+                                               int64_t ldv, const void *grad_out, int64_t ldg, const void *out,
+                                               int64_t ldo, const float *lse, int64_t num_edges, int64_t H,
+                                               int64_t head_dim, int dtype, float attn_drop, uint64_t seed,
+                                               uint64_t offset, float *beta_e, float *ds_e, void *stream_) {
+    const char *name = "pglb_dot_attn_bwd_edge_drop_x16";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    if (dtype == PGLB_DTYPE_BF16)
+        return dot_attn_bwd_edge_entry<__nv_bfloat16>(name, rows, cols, eid, q, ldq, k, ldk, v, ldv, grad_out, ldg, out,
+                                                      ldo, lse, num_edges, H, head_dim, beta_e, ds_e, stream_, &drop);
+    return dot_attn_bwd_edge_entry<__half>(name, rows, cols, eid, q, ldq, k, ldk, v, ldv, grad_out, ldg, out, ldo, lse,
+                                           num_edges, H, head_dim, beta_e, ds_e, stream_, &drop);
 }
 
 // The keep words of dst-CSR slots slot0 .. slot0 + n_slots - 1 on the host (include/pglb.h): the same attn_keep_word

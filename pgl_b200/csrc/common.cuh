@@ -124,6 +124,20 @@ __device__ __forceinline__ float4 ldg_row4(const T *p) {
     else return widen4<T>(__ldg(reinterpret_cast<const uint2 *>(p)));
 }
 
+// The score of the dot-product attention kernels (spmm_gat5_kernel<DOT>, dot_attn_bwd_edge_kernel): a lane's 4-term
+// partial dot, then the sum over the lph lanes of its head (lph a power of two, warp-uniform, every lane of the warp
+// calling).  The forward and the edge backward both call these two, so they form the same score bit for bit, and
+// every lane of a head holds the same bits.
+__device__ __forceinline__ float dot4_lane(const float4 &a, const float4 &b) {
+    return fmaf(a.w, b.w, fmaf(a.z, b.z, fmaf(a.y, b.y, a.x * b.x)));
+}
+__device__ __forceinline__ float head_sum_lanes(float v, int lph) {
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1)
+        if (o < lph) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
 // ---- attention dropout of the fused GAT training path (the *_drop_* entries) ----------------------------------------
 // The keep decision of dst-CSR slot j (absolute slot index) and head h, for drop probability p:
 //   draw = Philox4x32-10(counter = (j lo32, j hi32, h / 4, offset / 4), key = (seed lo32, seed hi32)) word h % 4

@@ -484,6 +484,14 @@ int gat_fused_run(const int64_t *indptr, const int64_t *cols, const void *f, int
                   size_t ws_bytes, cudaStream_t stream);
 template <typename T>
 bool gat5_takes(int64_t D, float slope, const void *f, int64_t ldf, const float *attn_src, int64_t H, int64_t n_src);
+// the fused dot-product attention (TransformerConv) over q / k / v / out of element type T, and whether it takes a call
+template <typename T>
+int dot_attn_run(const int64_t *indptr, const int64_t *cols, const void *q, int64_t ldq, const void *k, int64_t ldk,
+                 const void *v, int64_t ldv, void *out, int64_t ldo, float *lse, int64_t n_dst, int64_t E, int64_t H,
+                 int64_t head_dim, const AttnDrop *drop, void *ws, size_t ws_bytes, cudaStream_t stream);
+template <typename T>
+bool dot_attn_takes(int64_t D, int64_t head_dim, const void *q, int64_t ldq, const void *k, int64_t ldk, const void *v,
+                    int64_t ldv, int64_t n_src);
 
 // spmm_v5_kernel over rows of element type T (float, __nv_bfloat16 or __half): whether it takes a call, and the run
 template <typename T>
@@ -868,6 +876,91 @@ extern "C" int pglb_gat_fused_train_drop_csr_x16(const int64_t *indptr, const in
         using T = std::remove_pointer_t<decltype(elem)>;
         return gat_fused_entry<T>(name, indptr, cols, f, ldf, attn_src, attn_dst, negative_slope, out, ldo, lse, n_dst,
                                   n_src, num_edges, H, head_dim, ws, ws_bytes, stream_, &drop);
+    };
+    return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
+}
+
+// The argument checks and the launch of the dot-product attention entries (include/pglb.h).  T: element type of q, k,
+// v and out.  Every check precedes any CUDA call.  drop (nullable): the attention-dropout stream.
+template <typename T>
+static int dot_attn_entry(const char *name, const int64_t *indptr, const int64_t *cols, const void *q, int64_t ldq,
+                          const void *k, int64_t ldk, const void *v, int64_t ldv, void *out, int64_t ldo, float *lse,
+                          int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H, int64_t head_dim, void *ws,
+                          size_t ws_bytes, void *stream_, const AttnDrop *drop) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    constexpr int64_t B = sizeof(T);
+    PGLB_CHECK_ARG(n_dst >= 0 && n_src >= 0 && num_edges >= 0 && H > 0 && head_dim > 0, PGLB_EINVAL, "%s: bad size", name);
+    const int64_t D = H * head_dim;
+    const int64_t lph = head_dim / 4;
+    PGLB_CHECK_ARG(D <= 128 && head_dim % 4 == 0 && (lph & (lph - 1)) == 0 && (D * B) % 16 == 0 &&
+                       num_edges < 0x7fffffffLL && n_src < 0x7fffffffLL,
+                   PGLB_EUNSUPPORTED, "%s: needs H*head_dim <= 128 in 16-byte rows, head_dim in {4, 8, ..., 128}", name);
+    PGLB_CHECK_ARG(!drop || H % 4 == 0, PGLB_EUNSUPPORTED, "%s: attention dropout needs H %% 4 == 0", name);
+    if (n_dst == 0) return PGLB_OK;
+    PGLB_CHECK_ARG(indptr && out, PGLB_EINVAL, "%s: NULL pointer", name);
+    PGLB_CHECK_ARG(ldq >= D && ldk >= D && ldv >= D && ldo >= D && (ldo * B) % 16 == 0 && aligned16(out) &&
+                       dot_attn_takes<T>(D, head_dim, q, ldq, k, ldk, v, ldv, n_src),
+                   PGLB_ESHAPE, "%s: rows must be 16-byte aligned", name);
+    if (num_edges == 0) {
+        PGLB_CUDA(cudaMemset2DAsync(out, B * ldo, 0, B * D, n_dst, stream));
+        return PGLB_OK;
+    }
+    PGLB_CHECK_ARG(cols && q && k && v, PGLB_EINVAL, "%s: NULL pointer", name);
+    PGLB_CHECK_ARG(ws && (reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
+                   "%s: workspace NULL or not 256-byte aligned", name);
+    return dot_attn_run<T>(indptr, cols, q, ldq, k, ldk, v, ldv, out, ldo, lse, n_dst, num_edges, H, head_dim, drop, ws,
+                           ws_bytes, stream);
+}
+
+extern "C" int pglb_dot_attn_csr_f32(const int64_t *indptr, const int64_t *cols, const float *q, int64_t ldq,
+                                     const float *k, int64_t ldk, const float *v, int64_t ldv, float *out, int64_t ldo,
+                                     float *lse, int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H,
+                                     int64_t head_dim, void *ws, size_t ws_bytes, void *stream_) {
+    return dot_attn_entry<float>("pglb_dot_attn_csr_f32", indptr, cols, q, ldq, k, ldk, v, ldv, out, ldo, lse, n_dst,
+                                 n_src, num_edges, H, head_dim, ws, ws_bytes, stream_, nullptr);
+}
+
+extern "C" int pglb_dot_attn_csr_x16(const int64_t *indptr, const int64_t *cols, const void *q, int64_t ldq,
+                                     const void *k, int64_t ldk, const void *v, int64_t ldv, void *out, int64_t ldo,
+                                     float *lse, int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H,
+                                     int64_t head_dim, int dtype, void *ws, size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_dot_attn_csr_x16";
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    auto run = [&](auto *elem) -> int {
+        using T = std::remove_pointer_t<decltype(elem)>;
+        return dot_attn_entry<T>(name, indptr, cols, q, ldq, k, ldk, v, ldv, out, ldo, lse, n_dst, n_src, num_edges, H,
+                                 head_dim, ws, ws_bytes, stream_, nullptr);
+    };
+    return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
+}
+
+extern "C" int pglb_dot_attn_drop_csr_f32(const int64_t *indptr, const int64_t *cols, const float *q, int64_t ldq,
+                                          const float *k, int64_t ldk, const float *v, int64_t ldv, float *out,
+                                          int64_t ldo, float *lse, int64_t n_dst, int64_t n_src, int64_t num_edges,
+                                          int64_t H, int64_t head_dim, float attn_drop, uint64_t seed, uint64_t offset,
+                                          void *ws, size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_dot_attn_drop_csr_f32";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    return dot_attn_entry<float>(name, indptr, cols, q, ldq, k, ldk, v, ldv, out, ldo, lse, n_dst, n_src, num_edges, H,
+                                 head_dim, ws, ws_bytes, stream_, &drop);
+}
+
+extern "C" int pglb_dot_attn_drop_csr_x16(const int64_t *indptr, const int64_t *cols, const void *q, int64_t ldq,
+                                          const void *k, int64_t ldk, const void *v, int64_t ldv, void *out,
+                                          int64_t ldo, float *lse, int64_t n_dst, int64_t n_src, int64_t num_edges,
+                                          int64_t H, int64_t head_dim, int dtype, float attn_drop, uint64_t seed,
+                                          uint64_t offset, void *ws, size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_dot_attn_drop_csr_x16";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    auto run = [&](auto *elem) -> int {
+        using T = std::remove_pointer_t<decltype(elem)>;
+        return dot_attn_entry<T>(name, indptr, cols, q, ldq, k, ldk, v, ldv, out, ldo, lse, n_dst, n_src, num_edges, H,
+                                 head_dim, ws, ws_bytes, stream_, &drop);
     };
     return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
 }

@@ -1246,7 +1246,44 @@ int gat_fused_run(const int64_t *indptr, const int64_t *cols, const void *f, int
     return PGLB_EUNSUPPORTED;   // not reached: refused above
 }
 
+template <typename T>
+bool dot_attn_takes(int64_t D, int64_t head_dim, const void *q, int64_t ldq, const void *k, int64_t ldk, const void *v,
+                    int64_t ldv, int64_t n_src) {
+    return dot_attn_eligible<T>(D, head_dim, q, ldq, k, ldk, v, ldv, n_src);
+}
+
+// Single-pass dot-product attention (TransformerConv): out[d,h,:] = sum_j softmax_j(<q[d,h,:], k[src_j,h,:]>) v[src_j,h,:]
+// on spmm_gat5_kernel<DOT>.  T: element type of q, k, v and out; the call is one dot_attn_takes accepts.  lse
+// (nullable): the rows' log-sum-exp.  drop (nullable): the attention-dropout stream.
+template <typename T>
+int dot_attn_run(const int64_t *indptr, const int64_t *cols, const void *q, int64_t ldq, const void *k, int64_t ldk,
+                 const void *v, int64_t ldv, void *out, int64_t ldo, float *lse, int64_t n_dst, int64_t E, int64_t H,
+                 int64_t head_dim, const AttnDrop *drop, void *ws, size_t ws_bytes, cudaStream_t stream) {
+    StreamP p{};
+    p.ldy = H;
+    p.head_dim = (int)head_dim;
+    p.lse = lse;
+    {
+        const int rc = stream_prepare(p, gat_task_size(E), indptr, cols, v, ldv, out, ldo, n_dst, E, H * head_dim,
+                                      PGLB_REDUCE_SUM, nullptr, nullptr, nullptr, nullptr, ws, ws_bytes, stream);
+        if (rc) return rc;
+    }
+    p.dyn = dyn_mode("PGLB_GAT_DYN", 1, p.ntasks);
+    {
+        const int rc = launch_empty_rows<T>(p, stream);
+        if (rc) return rc;
+    }
+    if (drop) return launch_dot_attn<T, true>(p, q, ldq, k, ldk, *drop, stream);
+    return launch_dot_attn<T, false>(p, q, ldq, k, ldk, AttnDrop{}, stream);
+}
+
 // the instantiations the entries in spmm.cu call
+template decltype(dot_attn_takes<float>) dot_attn_takes<float>;
+template decltype(dot_attn_takes<__nv_bfloat16>) dot_attn_takes<__nv_bfloat16>;
+template decltype(dot_attn_takes<__half>) dot_attn_takes<__half>;
+template decltype(dot_attn_run<float>) dot_attn_run<float>;
+template decltype(dot_attn_run<__nv_bfloat16>) dot_attn_run<__nv_bfloat16>;
+template decltype(dot_attn_run<__half>) dot_attn_run<__half>;
 template decltype(gat5_takes<__nv_bfloat16>) gat5_takes<__nv_bfloat16>;
 template decltype(gat5_takes<__half>) gat5_takes<__half>;
 template decltype(gat_fused_run<float>) gat_fused_run<float>;
