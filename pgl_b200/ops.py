@@ -897,11 +897,14 @@ class _MaxMinAgg(torch.autograd.Function):
             # widening is exact, so the fp32 kernel's equality test x == out picks the same entries
             x2, out, g = x2.float(), out.float(), g.float()
         g = g.contiguous()
-        gx = torch.empty_like(x2)
+        # as in _CopyAgg.backward: feature rows past the graph's nodes are never gathered, so they get zero gradient;
+        # the kernel only walks the rows the reverse CSR has
+        n_src = int(x2.shape[0])
+        rows = min(n_src, int(bwd["indptr"].shape[0]) - 1)
+        gx = torch.zeros_like(x2) if rows < n_src else torch.empty_like(x2)
         with torch.cuda.device(x2.device):
             check(lib.pglb_maxmin_bwd_f32(_ptr(bwd["indptr"]), _ptr(bwd["cols"]), _ptr(x2), _ptr(out),
-                                          _ptr(g), _ptr(gx), int(x2.shape[0]), int(x2.shape[1]),
-                                          _stream()))
+                                          _ptr(g), _ptr(gx), rows, int(x2.shape[1]), _stream()))
         return gx.to(dtype), None, None, None, None
 
 
