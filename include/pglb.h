@@ -464,6 +464,91 @@ int pglb_dot_attn_bwd_edge_drop_x16(const int64_t *rows, const int64_t *cols, co
                                     float attn_drop, uint64_t seed, uint64_t offset, float *beta_e, float *ds_e,
                                     void *stream);
 
+/* GATv2 attention (pgl/nn/conv.py:420-427: send_uv(feature, feature, add), LeakyReLU, the sum with attn over the head
+ * dim, edge_softmax, attention dropout, send_ue_recv(mul, sum)) in ONE pass, the GAT kernel's online softmax:
+ *   z_j = f[cols[j],h,:] + f[d,h,:],  s_j = sum_c a[h,c] lrelu(z_j,c),  lrelu(x) = max(x, slope x),
+ *   lse[d,h] = log sum_j exp(s_j),  out[d,h,:] = sum_j exp(s_j - lse) f[cols[j],h,:]
+ * over the dst-CSR slots j of row d (rows without in-edges: out = 0).  No [E, H * head_dim] tensor is ever written.
+ *   - f [n, H * head_dim] with row stride ldf, out [n, ...] with row stride ldo, in elements; attn = a, H * head_dim
+ *     float32.  lse [n, H] float32 is nullable (inference); when given, rows with at least one in-edge are written
+ *     (others are not).  ws as pglb_spmm_csr_ws(n, num_edges, H * head_dim).
+ *   - Shapes: D = H * head_dim <= 128 in 16-byte rows (D % 4 == 0 float32, D % 8 == 0 16-bit), head_dim in
+ *     {4, 8, ..., 128}, 0 <= negative_slope <= 1, n < 2^31 - 1: otherwise PGLB_EUNSUPPORTED.  f, attn, out not 16-byte
+ *     aligned, a row stride below D or not a multiple of 16 bytes: PGLB_ESHAPE.
+ *   - _x16 (`dtype` bfloat16 / float16 f and out; attn and lse float32): rows are widened exactly and every later
+ *     operation is the float32 kernel's in the same slot order, rounded once on the store, so out ==
+ *     round16(pglb_gatv2_attn_csr_f32 on the widened f) and lse equals its lse, bit for bit.  Unknown dtype: PGLB_EINVAL.
+ *   - _drop_ (attention dropout): attn_drop, seed, offset with the stream and rules of the GAT dropout entries above
+ *     (same keep word per dst-CSR slot and head, H % 4 == 0): out = sum_j s m_j exp(s_j - lse) f[cols[j]], and lse is
+ *     bitwise the value without dropout.
+ *   - All argument checks precede any CUDA call. */
+int pglb_gatv2_attn_csr_f32(const int64_t *indptr, const int64_t *cols, const float *f, int64_t ldf, const float *attn,
+                            float negative_slope, float *out, int64_t ldo, float *lse, int64_t n, int64_t num_edges,
+                            int64_t H, int64_t head_dim, void *ws, size_t ws_bytes, void *stream);
+int pglb_gatv2_attn_csr_x16(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf, const float *attn,
+                            float negative_slope, void *out, int64_t ldo, float *lse, int64_t n, int64_t num_edges,
+                            int64_t H, int64_t head_dim, int dtype, void *ws, size_t ws_bytes, void *stream);
+int pglb_gatv2_attn_drop_csr_f32(const int64_t *indptr, const int64_t *cols, const float *f, int64_t ldf,
+                                 const float *attn, float negative_slope, float *out, int64_t ldo, float *lse, int64_t n,
+                                 int64_t num_edges, int64_t H, int64_t head_dim, float attn_drop, uint64_t seed,
+                                 uint64_t offset, void *ws, size_t ws_bytes, void *stream);
+int pglb_gatv2_attn_drop_csr_x16(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
+                                 const float *attn, float negative_slope, void *out, int64_t ldo, float *lse, int64_t n,
+                                 int64_t num_edges, int64_t H, int64_t head_dim, int dtype, float attn_drop,
+                                 uint64_t seed, uint64_t offset, void *ws, size_t ws_bytes, void *stream);
+
+/* Per-edge part of that attention's backward.  rows / cols / eid as pglb_gat_bwd_edge_f32; lse from the forward;
+ * grad_out = G.  With s and a = exp(s - lse[dst,h]) rebuilt (s bit for bit the forward's score):
+ *   beta_e[e,h] = a,   ds_e[e,h] = a * (<G[dst,h,:], f[src,h,:]> - <G[dst,h,:], out[dst,h,:]>)
+ * both [num_edges, H] float32 in ORIGINAL edge order.  grad_attn (nullable, H * head_dim float32) receives
+ * grad a[h,c] = sum_e ds_e[e,h] lrelu(z_e,c), reduced in a fixed order (bit-identical run to run) through ws
+ * (pglb_gatv2_bwd_edge_ws bytes, 16-byte aligned; unused when grad_attn is NULL).  The caller finishes grad f with
+ * pglb_gatv2_score_grad_* on the dst-keyed and the src-keyed CSR and send_ue_recv(grad_out, beta_e, mul, sum) over
+ * the src-keyed CSR.  Shapes as the forward's: otherwise PGLB_EUNSUPPORTED.
+ *   - _x16: f, grad_out and out in `dtype`, widened exactly; beta_e, ds_e and grad_attn equal the f32 entry's on the
+ *     widened inputs bit for bit.
+ *   - _drop_: the forward's attn_drop, seed, offset; da is multiplied by s m, and beta_e = m ? fl(a * s) : 0. */
+int pglb_gatv2_bwd_edge_ws(int64_t num_edges, size_t *ws_bytes);
+int pglb_gatv2_bwd_edge_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *f, int64_t ldf,
+                            const float *attn, float negative_slope, const float *grad_out, int64_t ldg,
+                            const float *out, int64_t ldo, const float *lse, int64_t num_edges, int64_t H,
+                            int64_t head_dim, float *beta_e, float *ds_e, float *grad_attn, void *ws, size_t ws_bytes,
+                            void *stream);
+int pglb_gatv2_bwd_edge_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *f, int64_t ldf,
+                            const float *attn, float negative_slope, const void *grad_out, int64_t ldg, const void *out,
+                            int64_t ldo, const float *lse, int64_t num_edges, int64_t H, int64_t head_dim, int dtype,
+                            float *beta_e, float *ds_e, float *grad_attn, void *ws, size_t ws_bytes, void *stream);
+int pglb_gatv2_bwd_edge_drop_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *f,
+                                 int64_t ldf, const float *attn, float negative_slope, const float *grad_out,
+                                 int64_t ldg, const float *out, int64_t ldo, const float *lse, int64_t num_edges,
+                                 int64_t H, int64_t head_dim, float attn_drop, uint64_t seed, uint64_t offset,
+                                 float *beta_e, float *ds_e, float *grad_attn, void *ws, size_t ws_bytes,
+                                 void *stream);
+int pglb_gatv2_bwd_edge_drop_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *f,
+                                 int64_t ldf, const float *attn, float negative_slope, const void *grad_out,
+                                 int64_t ldg, const void *out, int64_t ldo, const float *lse, int64_t num_edges,
+                                 int64_t H, int64_t head_dim, int dtype, float attn_drop, uint64_t seed,
+                                 uint64_t offset, float *beta_e, float *ds_e, float *grad_attn, void *ws,
+                                 size_t ws_bytes, void *stream);
+
+/* The score-gradient aggregation of that backward:
+ *   out[r, c] (+)= sum over the slots j of row r of ds[eid[j], h(c)] * attn[c] * lrelu'(f[r, c] + f[cols[j], c])
+ * lrelu'(x) = 1 if x > 0 else negative_slope (torch's convention at 0).  On the dst-keyed CSR it is the dst term of
+ * grad f, on the src-keyed CSR the src term; the [E, H * head_dim] dz is recomputed, never stored.  ds [E, H] float32
+ * from pglb_gatv2_bwd_edge_*, eid nullable (identity).  out float32 [n_rows, H * head_dim], row stride ldo; accumulate:
+ * add out's previous contents.  Every row's sum runs in slot order (rows longer than 1024 slots in fixed 1024-slot
+ * chunks, summed in chunk order) with no atomics: bit-identical run to run.  ws as pglb_spmm_csr_ws(n_rows,
+ * num_edges, H * head_dim).  D <= 128 in 16-byte rows, head_dim % 4 == 0, 0 <= negative_slope <= 1: otherwise
+ * PGLB_EUNSUPPORTED; f, attn, out not 16-byte aligned: PGLB_ESHAPE.  _x16: f in `dtype`, widened exactly. */
+int pglb_gatv2_score_grad_f32(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const float *f,
+                              int64_t ldf, const float *attn, float negative_slope, const float *ds, float *out,
+                              int64_t ldo, int64_t n_rows, int64_t num_edges, int64_t H, int64_t head_dim,
+                              int accumulate, void *ws, size_t ws_bytes, void *stream);
+int pglb_gatv2_score_grad_x16(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const void *f,
+                              int64_t ldf, const float *attn, float negative_slope, const float *ds, float *out,
+                              int64_t ldo, int64_t n_rows, int64_t num_edges, int64_t H, int64_t head_dim, int dtype,
+                              int accumulate, void *ws, size_t ws_bytes, void *stream);
+
 /* out[M, N] = act(x[M, K] @ w[K, N] + bias[N]) -- the dense transform of the conv layers
  * (pgl/nn/conv.py:238-251 GCNConv: `self.linear(...)`, `+ self.bias`, activation; the same Linear in
  * GATConv :321 / GraphSageConv :107-108) on the tensor cores with 3xTF32 error compensation (fp32-level

@@ -283,6 +283,121 @@ __global__ void __launch_bounds__(256) dot_attn_bwd_edge_kernel(
     }
 }
 
+// Backward of the single-pass GATv2 attention (pglb_gatv2_attn_*), the per-edge part, on dot_attn_bwd_edge_kernel's
+// walk.  With z = f[src,h,:] + f[dst,h,:], s = sum_c a[h,c] lrelu(z_c), a = exp(s - lse[dst,h]), G = d loss / d out:
+//   da = <G[dst,h,:], f[src,h,:]>,   delta = <G[dst,h,:], out[dst,h,:]>,   ds = a (da - delta)
+// written, with beta = a, as [E, H] fp32 in ORIGINAL edge order.  s is formed by the forward's gatv2_lane +
+// head_sum_lanes, so it is the forward's score bit for bit.  ga_part (nullable): grad a = sum_e ds lrelu(z), each block's
+// share (its warps' lane sums added in warp order) at ga_part[blockIdx.x * 128 ...]; gatv2_ga_reduce_kernel adds the
+// blocks in order.  The grid is fixed, so grad a is bit-identical run to run.  T: element type of f, G and out.
+// DROP: da = s m da and beta = m ? fl(a s) : 0 (m the slot and head's keep bit, s = 1 / (1 - p)); delta is unchanged.
+template <int LPH, typename T, bool DROP>
+__global__ void __launch_bounds__(256) gatv2_bwd_edge_kernel(
+    const int64_t *__restrict__ rows, const int64_t *__restrict__ cols, const int64_t *__restrict__ eid,
+    const T *__restrict__ f, int64_t ldf, const float *__restrict__ attn, float slope, const T *__restrict__ g,
+    int64_t ldg, const T *__restrict__ out, int64_t ldo, const float *__restrict__ lse, int64_t E, int H, int D,
+    float *__restrict__ beta_e, float *__restrict__ ds_e, float *__restrict__ ga_part, const AttnDrop drop) {
+    __shared__ float4 ga_warp[8][32];
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const bool act = lane * 4 < D;
+    const int head = act ? lane / LPH : 0;
+    const bool lead = act && (lane % LPH) == 0;
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 a4 = act ? __ldg(reinterpret_cast<const float4 *>(attn) + lane) : zero;
+    float4 ga = zero;
+    for (int64_t base = warp * 32; base < E; base += nwarps * 32) {
+        const int64_t j = base + lane;
+        const bool in = j < E;
+        const long long r_l = in ? ld_stream(rows + j) : 0;
+        const long long c_l = in ? ld_stream(cols + j) : 0;
+        const long long i_l = in ? (eid ? ld_stream(eid + j) : j) : 0;
+        unsigned kw_l = 0;
+        if constexpr (DROP) kw_l = attn_keep_word(drop, (uint64_t)j, H);
+        const int cnt = (E - base) < 32 ? (int)(E - base) : 32;
+        long long cur = -1;
+        float4 fd = zero, g4 = zero;
+        float ls = 0.f, delta = 0.f;
+        for (int k0 = 0; k0 < cnt; k0 += 4) {
+            float4 fs[4];
+            long long rr[4], ii[4];
+            unsigned kk[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const int s = (k0 + u) & 31;
+                const long long cc = __shfl_sync(0xffffffffu, c_l, s);
+                rr[u] = __shfl_sync(0xffffffffu, r_l, s);
+                ii[u] = __shfl_sync(0xffffffffu, i_l, s);
+                if constexpr (DROP) kk[u] = __shfl_sync(0xffffffffu, kw_l, s);
+                fs[u] = zero;
+                if (k0 + u < cnt && act) fs[u] = ldg_row4<T>(f + cc * ldf + lane * 4);
+            }
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                if (k0 + u >= cnt) break;
+                if (rr[u] != cur) {  // warp-uniform
+                    cur = rr[u];
+                    float d = 0.f;
+                    if (act) {
+                        fd = ldg_row4<T>(f + cur * ldf + lane * 4);
+                        g4 = ldg_row4<T>(g + cur * ldg + lane * 4);
+                        d = dot4_lane(g4, ldg_row4<T>(out + cur * ldo + lane * 4));
+                        ls = __ldg(lse + cur * H + head);
+                    }
+                    delta = head_sum_lanes(d, LPH);
+                }
+                const float sc = head_sum_lanes(gatv2_lane(a4, fs[u], fd, slope), LPH);
+                float da = head_sum_lanes(dot4_lane(g4, fs[u]), LPH);
+                const float a = expf(sc - ls);
+                float beta = a;
+                if constexpr (DROP) {
+                    const bool keep = (kk[u] >> head) & 1u;
+                    da = keep ? drop.scale * da : 0.f;
+                    beta = keep ? a * drop.scale : 0.f;
+                }
+                const float ds = a * (da - delta);
+                if (lead) {
+                    beta_e[ii[u] * H + head] = beta;
+                    ds_e[ii[u] * H + head] = ds;
+                }
+                ga.x = fmaf(ds, lrelu_of(fs[u].x + fd.x, slope), ga.x);
+                ga.y = fmaf(ds, lrelu_of(fs[u].y + fd.y, slope), ga.y);
+                ga.z = fmaf(ds, lrelu_of(fs[u].z + fd.z, slope), ga.z);
+                ga.w = fmaf(ds, lrelu_of(fs[u].w + fd.w, slope), ga.w);
+            }
+        }
+    }
+    if (ga_part == nullptr) return;   // uniform over the grid
+    ga_warp[threadIdx.x >> 5][lane] = ga;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        float4 t = ga_warp[0][lane];
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) {
+            const float4 v = ga_warp[w][lane];
+            t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w;
+        }
+        reinterpret_cast<float4 *>(ga_part + (int64_t)blockIdx.x * 128)[lane] = t;
+    }
+}
+
+// grad a[c] = sum over the nb blocks' shares ga_part[b * 128 + c], in a fixed order: block c of the grid, thread t adds
+// b = t, t + 256, ..., then a fixed tree over the threads.
+__global__ void __launch_bounds__(256) gatv2_ga_reduce_kernel(const float *__restrict__ ga_part, int nb,
+                                                              float *__restrict__ grad_attn) {
+    __shared__ float red[256];
+    const int c = blockIdx.x, t = threadIdx.x;
+    float v = 0.f;
+    for (int b = t; b < nb; b += 256) v += ga_part[(int64_t)b * 128 + c];
+    red[t] = v;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (t < o) red[t] += red[t + o];
+        __syncthreads();
+    }
+    if (t == 0) grad_attn[c] = red[0];
+}
+
 static inline int grid_of(int64_t total, int cap_mult) {
     int64_t b = (total + 255) / 256;
     const int64_t cap = (int64_t)sm_count() * cap_mult;
@@ -555,6 +670,138 @@ extern "C" int pglb_dot_attn_bwd_edge_drop_x16(const int64_t *rows, const int64_
                                                       ldo, lse, num_edges, H, head_dim, beta_e, ds_e, stream_, &drop);
     return dot_attn_bwd_edge_entry<__half>(name, rows, cols, eid, q, ldq, k, ldk, v, ldv, grad_out, ldg, out, ldo, lse,
                                            num_edges, H, head_dim, beta_e, ds_e, stream_, &drop);
+}
+
+// The checks and the launch of the GATv2 edge-backward entries (include/pglb.h).  T: element type of f, grad_out and
+// out, rows 16-byte aligned.  drop (nullable): the attention-dropout stream (H % 4 == 0 then).
+static size_t gatv2_bwd_edge_ws_bytes(int64_t num_edges) { return (size_t)grid_of(num_edges, 64) * 128 * 4; }
+
+template <typename T>
+static int gatv2_bwd_edge_entry(const char *name, const int64_t *rows, const int64_t *cols, const int64_t *eid,
+                                const void *f_, int64_t ldf, const float *attn, float slope, const void *g_,
+                                int64_t ldg, const void *out_, int64_t ldo, const float *lse, int64_t num_edges,
+                                int64_t H, int64_t head_dim, float *beta_e, float *ds_e, float *grad_attn, void *ws,
+                                size_t ws_bytes, void *stream_, const AttnDrop *drop) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    const T *f = reinterpret_cast<const T *>(f_), *g = reinterpret_cast<const T *>(g_),
+            *out = reinterpret_cast<const T *>(out_);
+    constexpr int64_t B = sizeof(T);
+    PGLB_CHECK_ARG(num_edges >= 0 && H > 0 && head_dim > 0, PGLB_EINVAL, "%s: bad size", name);
+    const int64_t D = H * head_dim;
+    const int64_t lph = head_dim / 4;
+    PGLB_CHECK_ARG(D <= 128 && head_dim % 4 == 0 && (lph & (lph - 1)) == 0 && (D * B) % 16 == 0, PGLB_EUNSUPPORTED,
+                   "%s: needs H*head_dim <= 128 in 16-byte rows and head_dim in {4, 8, 16, 32, 64, 128}", name);
+    PGLB_CHECK_ARG(slope >= 0.0f && slope <= 1.0f, PGLB_EUNSUPPORTED, "%s: needs 0 <= negative_slope <= 1", name);
+    PGLB_CHECK_ARG(!drop || H % 4 == 0, PGLB_EUNSUPPORTED, "%s: needs H %% 4 == 0", name);
+    if (num_edges == 0) {
+        if (grad_attn) PGLB_CUDA(cudaMemsetAsync(grad_attn, 0, sizeof(float) * D, stream));
+        return PGLB_OK;
+    }
+    PGLB_CHECK_ARG(rows && cols && f && attn && g && out && lse && beta_e && ds_e, PGLB_EINVAL, "%s: NULL pointer",
+                   name);
+    auto a16 = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
+    PGLB_CHECK_ARG(ldf >= D && ldg >= D && ldo >= D && (ldf * B) % 16 == 0 && (ldg * B) % 16 == 0 &&
+                       (ldo * B) % 16 == 0 && a16(f) && a16(g) && a16(out) && a16(attn),
+                   PGLB_ESHAPE, "%s: rows must be 16-byte aligned", name);
+    PGLB_CHECK_ARG(!grad_attn || (ws && ws_bytes >= gatv2_bwd_edge_ws_bytes(num_edges) && a16(ws)), PGLB_EWORKSPACE,
+                   "%s: workspace of %zu bytes needed (got %zu)", name, gatv2_bwd_edge_ws_bytes(num_edges), ws_bytes);
+    const int grid = grid_of(num_edges, 64);  // a warp per 32 slots, grid-stride
+    const AttnDrop dr = drop ? *drop : AttnDrop{};
+    float *ga_part = grad_attn ? reinterpret_cast<float *>(ws) : nullptr;
+#define PGLB_V2E(L)                                                                                                   \
+    do {                                                                                                              \
+        if (drop)                                                                                                     \
+            gatv2_bwd_edge_kernel<L, T, true><<<grid, 256, 0, stream>>>(rows, cols, eid, f, ldf, attn, slope, g, ldg, \
+                                                                        out, ldo, lse, num_edges, (int)H, (int)D,     \
+                                                                        beta_e, ds_e, ga_part, dr);                   \
+        else                                                                                                          \
+            gatv2_bwd_edge_kernel<L, T, false><<<grid, 256, 0, stream>>>(rows, cols, eid, f, ldf, attn, slope, g,     \
+                                                                         ldg, out, ldo, lse, num_edges, (int)H,       \
+                                                                         (int)D, beta_e, ds_e, ga_part, dr);          \
+    } while (0)
+    switch ((int)lph) {
+        case 1: PGLB_V2E(1); break;
+        case 2: PGLB_V2E(2); break;
+        case 4: PGLB_V2E(4); break;
+        case 8: PGLB_V2E(8); break;
+        case 16: PGLB_V2E(16); break;
+        default: PGLB_V2E(32); break;
+    }
+#undef PGLB_V2E
+    PGLB_LAUNCH_CHECK("gatv2_bwd_edge_kernel");
+    if (grad_attn) {
+        gatv2_ga_reduce_kernel<<<(unsigned)D, 256, 0, stream>>>(ga_part, grid, grad_attn);
+        PGLB_LAUNCH_CHECK("gatv2_ga_reduce_kernel");
+    }
+    return PGLB_OK;
+}
+
+extern "C" int pglb_gatv2_bwd_edge_ws(int64_t num_edges, size_t *ws_bytes) {
+    PGLB_CHECK_ARG(ws_bytes != nullptr, PGLB_EINVAL, "pglb_gatv2_bwd_edge_ws: ws_bytes is NULL");
+    PGLB_CHECK_ARG(num_edges >= 0, PGLB_EINVAL, "pglb_gatv2_bwd_edge_ws: negative size");
+    *ws_bytes = gatv2_bwd_edge_ws_bytes(num_edges);
+    return PGLB_OK;
+}
+
+extern "C" int pglb_gatv2_bwd_edge_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *f,
+                                       int64_t ldf, const float *attn, float negative_slope, const float *grad_out,
+                                       int64_t ldg, const float *out, int64_t ldo, const float *lse, int64_t num_edges,
+                                       int64_t H, int64_t head_dim, float *beta_e, float *ds_e, float *grad_attn,
+                                       void *ws, size_t ws_bytes, void *stream_) {
+    return gatv2_bwd_edge_entry<float>("pglb_gatv2_bwd_edge_f32", rows, cols, eid, f, ldf, attn, negative_slope,
+                                       grad_out, ldg, out, ldo, lse, num_edges, H, head_dim, beta_e, ds_e, grad_attn,
+                                       ws, ws_bytes, stream_, nullptr);
+}
+
+extern "C" int pglb_gatv2_bwd_edge_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *f,
+                                       int64_t ldf, const float *attn, float negative_slope, const void *grad_out,
+                                       int64_t ldg, const void *out, int64_t ldo, const float *lse, int64_t num_edges,
+                                       int64_t H, int64_t head_dim, int dtype, float *beta_e, float *ds_e,
+                                       float *grad_attn, void *ws, size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_gatv2_bwd_edge_x16";
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    if (dtype == PGLB_DTYPE_BF16)
+        return gatv2_bwd_edge_entry<__nv_bfloat16>(name, rows, cols, eid, f, ldf, attn, negative_slope, grad_out, ldg,
+                                                   out, ldo, lse, num_edges, H, head_dim, beta_e, ds_e, grad_attn, ws,
+                                                   ws_bytes, stream_, nullptr);
+    return gatv2_bwd_edge_entry<__half>(name, rows, cols, eid, f, ldf, attn, negative_slope, grad_out, ldg, out, ldo,
+                                        lse, num_edges, H, head_dim, beta_e, ds_e, grad_attn, ws, ws_bytes, stream_,
+                                        nullptr);
+}
+
+extern "C" int pglb_gatv2_bwd_edge_drop_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid,
+                                            const float *f, int64_t ldf, const float *attn, float negative_slope,
+                                            const float *grad_out, int64_t ldg, const float *out, int64_t ldo,
+                                            const float *lse, int64_t num_edges, int64_t H, int64_t head_dim,
+                                            float attn_drop, uint64_t seed, uint64_t offset, float *beta_e,
+                                            float *ds_e, float *grad_attn, void *ws, size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_gatv2_bwd_edge_drop_f32";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    return gatv2_bwd_edge_entry<float>(name, rows, cols, eid, f, ldf, attn, negative_slope, grad_out, ldg, out, ldo,
+                                       lse, num_edges, H, head_dim, beta_e, ds_e, grad_attn, ws, ws_bytes, stream_,
+                                       &drop);
+}
+
+extern "C" int pglb_gatv2_bwd_edge_drop_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid,
+                                            const void *f, int64_t ldf, const float *attn, float negative_slope,
+                                            const void *grad_out, int64_t ldg, const void *out, int64_t ldo,
+                                            const float *lse, int64_t num_edges, int64_t H, int64_t head_dim,
+                                            int dtype, float attn_drop, uint64_t seed, uint64_t offset, float *beta_e,
+                                            float *ds_e, float *grad_attn, void *ws, size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_gatv2_bwd_edge_drop_x16";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    if (dtype == PGLB_DTYPE_BF16)
+        return gatv2_bwd_edge_entry<__nv_bfloat16>(name, rows, cols, eid, f, ldf, attn, negative_slope, grad_out, ldg,
+                                                   out, ldo, lse, num_edges, H, head_dim, beta_e, ds_e, grad_attn, ws,
+                                                   ws_bytes, stream_, &drop);
+    return gatv2_bwd_edge_entry<__half>(name, rows, cols, eid, f, ldf, attn, negative_slope, grad_out, ldg, out, ldo,
+                                        lse, num_edges, H, head_dim, beta_e, ds_e, grad_attn, ws, ws_bytes, stream_,
+                                        &drop);
 }
 
 // The keep words of dst-CSR slots slot0 .. slot0 + n_slots - 1 on the host (include/pglb.h): the same attn_keep_word

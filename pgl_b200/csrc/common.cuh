@@ -138,6 +138,16 @@ __device__ __forceinline__ float head_sum_lanes(float v, int lph) {
     return v;
 }
 
+// The GATv2 score (spmm_gat5_kernel<kScoreV2>, gatv2_bwd_edge_kernel, gatv2_score_grad_kernel): a lane's 4-term
+// partial sum_c a_c lrelu(fs_c + fd_c), then head_sum_lanes over its head.  lrelu(x) = max(x, slope x) for
+// 0 <= slope <= 1.  The forward and the edge backward call the same function, so they form the same score bit for bit.
+__device__ __forceinline__ float lrelu_of(float x, float slope) { return fmaxf(x, x * slope); }
+__device__ __forceinline__ float gatv2_lane(const float4 &a, const float4 &fs, const float4 &fd, float slope) {
+    return fmaf(a.w, lrelu_of(fs.w + fd.w, slope),
+                fmaf(a.z, lrelu_of(fs.z + fd.z, slope),
+                     fmaf(a.y, lrelu_of(fs.y + fd.y, slope), a.x * lrelu_of(fs.x + fd.x, slope))));
+}
+
 // ---- attention dropout of the fused GAT training path (the *_drop_* entries) ----------------------------------------
 // The keep decision of dst-CSR slot j (absolute slot index) and head h, for drop probability p:
 //   draw = Philox4x32-10(counter = (j lo32, j hi32, h / 4, offset / 4), key = (seed lo32, seed hi32)) word h % 4

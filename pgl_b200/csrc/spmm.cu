@@ -493,6 +493,15 @@ template <typename T>
 bool dot_attn_takes(int64_t D, int64_t head_dim, const void *q, int64_t ldq, const void *k, int64_t ldk, const void *v,
                     int64_t ldv, int64_t n_src);
 
+// the fused GATv2 attention (GATv2Conv) over f / out of element type T, and whether it takes a call
+template <typename T>
+int gatv2_attn_run(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf, const float *attn,
+                   float slope, void *out, int64_t ldo, float *lse, int64_t n, int64_t E, int64_t H, int64_t head_dim,
+                   const AttnDrop *drop, void *ws, size_t ws_bytes, cudaStream_t stream);
+template <typename T>
+bool gatv2_attn_takes(int64_t D, int64_t head_dim, float slope, const void *f, int64_t ldf, const float *attn,
+                      int64_t n_src);
+
 // spmm_v5_kernel over rows of element type T (float, __nv_bfloat16 or __half): whether it takes a call, and the run
 template <typename T>
 bool v5_eligible(const int64_t *cols, const uint32_t *cols32, const void *x, int64_t ldx, const void *out, int64_t ldo,
@@ -615,6 +624,230 @@ static int spmm_generic_run(const int64_t *indptr, const int64_t *cols, const in
             if (blocks > max_blocks) blocks = max_blocks;
             dim3 grid((unsigned)blocks, (unsigned)s.tiles);
             pick_kernel<float, E>(s, 0, rk)<<<grid, kThreads, 0, stream>>>(p2);
+            PGLB_LAUNCH_CHECK("spmm_csr_kernel(hub pass 2)");
+        }
+    }
+    return PGLB_OK;
+}
+
+// ---- GATv2 score gradient (pglb_gatv2_score_grad_*) ------------------------------------------------------------------
+// gr[r, c] = sum over the slots j of row r of ds[eid_j, h(c)] * a[c] * lrelu'(f[r, c] + f[cols_j, c]),
+// lrelu'(x) = 1 if x > 0 else slope (torch's convention at 0).  On the dst-keyed CSR this is the dst term of GATv2's
+// grad f, on the src-keyed CSR its src term (z = f[src] + f[dst] either way); the [E, H*Dh] dz is never stored.  A
+// group of G lanes owns a row, a lane 4 columns; slots are taken in order, so each row's sum has a fixed order.  Rows
+// longer than HUB_T slots go through spmm_generic_run's hub path: the same kernel over HUB_CH-slot chunks into fp32
+// partials (chunks = 1: a chunk's own row is found in indptr), then the copy-sum spmm_csr_kernel over a hub's partials
+// in chunk order.  No atomics on values: run to run the result is bit-identical.
+struct V2GradP {
+    const int64_t *rbeg;    // row r covers slots [rbeg[r], rend[r])
+    const int64_t *rend;
+    const int64_t *indptr;  // chunks: the CSR, to find the row whose slots hold rbeg[r]
+    int64_t n_ind;          // its row count
+    const int64_t *cols;
+    const int64_t *eid;     // nullable: identity
+    const void *f;          // [n, D] of T
+    int64_t ldf;
+    const float *attn;      // [D]
+    const float *ds;        // [E, H]
+    float slope;
+    int H, D, head_dim;
+    float *out;
+    int64_t ldo;
+    int64_t n_rows;
+    const int64_t *n_rows_dev;  // nullable: overrides n_rows (chunks)
+    int chunks;
+    int accumulate;             // add out's previous contents (rows of the main pass)
+    int64_t hub_threshold;
+    unsigned long long *hub_count;
+    int64_t *hub_rows;
+};
+
+template <typename T, int G>
+__global__ void __launch_bounds__(kThreads) gatv2_score_grad_kernel(const V2GradP p) {
+    const int lane = threadIdx.x & 31;
+    const int gl = lane & (G - 1);
+    const unsigned gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (lane & ~(G - 1)));
+    const int64_t gid = (int64_t)blockIdx.x * (kThreads / G) + threadIdx.x / G;
+    const int64_t ngroups = (int64_t)gridDim.x * (kThreads / G);
+    const int64_t n_rows = p.n_rows_dev ? *p.n_rows_dev : p.n_rows;
+    const int c0 = gl * 4;
+    const bool act = c0 < p.D;
+    const int head = act ? c0 / p.head_dim : 0;
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 a4 = act ? __ldg(reinterpret_cast<const float4 *>(p.attn) + gl) : zero;
+    const T *f = reinterpret_cast<const T *>(p.f);
+    const float slope = p.slope;
+    for (int64_t r = gid; r < n_rows; r += ngroups) {
+        const int64_t beg = ld_ro(p.rbeg + r), end = ld_ro(p.rend + r);
+        if (end - beg > p.hub_threshold) {
+            if (gl == 0) p.hub_rows[atomicAdd(p.hub_count, 1ull)] = r;
+            continue;
+        }
+        int64_t row = r;
+        if (p.chunks) {   // the last row whose first slot is <= beg (rows of a chunk are never empty)
+            int64_t lo = 0, hi = p.n_ind;
+            while (hi - lo > 1) {
+                const int64_t mid = (lo + hi) >> 1;
+                if (ld_ro(p.indptr + mid) <= beg) lo = mid;
+                else hi = mid;
+            }
+            row = lo;
+        }
+        const float4 fr = act ? ldg_row4<T>(f + row * p.ldf + c0) : zero;
+        float4 acc = zero;
+        for (int64_t pos = beg; pos < end; pos += G) {
+            const int nb = (end - pos) < (int64_t)G ? (int)(end - pos) : G;
+            int64_t my_col = 0, my_e = 0;
+            if (gl < nb) {
+                my_col = ld_stream(p.cols + pos + gl);
+                my_e = p.eid ? ld_stream(p.eid + pos + gl) : (pos + gl);
+            }
+            for (int k0 = 0; k0 < nb; k0 += 4) {
+                float4 fs[4];
+                float dv[4];
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    const int src = (k0 + u) & (G - 1);
+                    const int64_t c = __shfl_sync(gmask, my_col, src, G);
+                    const int64_t e = __shfl_sync(gmask, my_e, src, G);
+                    fs[u] = zero;
+                    dv[u] = 0.f;
+                    if (k0 + u < nb && act) {
+                        fs[u] = ldg_row4<T>(f + c * p.ldf + c0);
+                        dv[u] = __ldg(p.ds + e * p.H + head);
+                    }
+                }
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    if (k0 + u >= nb) break;
+                    // dz = ds * a * lrelu'(z), z = f[row] + f[col] (the forward's f[src] + f[dst], addition commutes)
+                    const float zx = fr.x + fs[u].x, zy = fr.y + fs[u].y, zz = fr.z + fs[u].z, zw = fr.w + fs[u].w;
+                    const float tx = dv[u] * a4.x, ty = dv[u] * a4.y, tz = dv[u] * a4.z, tw = dv[u] * a4.w;
+                    acc.x = __fadd_rn(acc.x, zx > 0.f ? tx : tx * slope);
+                    acc.y = __fadd_rn(acc.y, zy > 0.f ? ty : ty * slope);
+                    acc.z = __fadd_rn(acc.z, zz > 0.f ? tz : tz * slope);
+                    acc.w = __fadd_rn(acc.w, zw > 0.f ? tw : tw * slope);
+                }
+            }
+        }
+        if (act) {
+            float *o = p.out + r * p.ldo + c0;
+            if (p.accumulate) {
+                const float4 prev = *reinterpret_cast<const float4 *>(o);
+                acc = make_float4(__fadd_rn(prev.x, acc.x), __fadd_rn(prev.y, acc.y), __fadd_rn(prev.z, acc.z),
+                                  __fadd_rn(prev.w, acc.w));
+            }
+            *reinterpret_cast<float4 *>(o) = acc;
+        }
+    }
+}
+
+template <typename T, int G>
+static void launch_v2_grad(const V2GradP &p, int64_t blocks, cudaStream_t stream) {
+    gatv2_score_grad_kernel<T, G><<<(unsigned)blocks, kThreads, 0, stream>>>(p);
+}
+
+// The launch sequence of pglb_gatv2_score_grad_*: main pass over the rows, then the hub plan and the two hub passes
+// when some row is longer than HUB_T slots.  out is float32 [n_rows, D]; ws as pglb_spmm_csr_ws(n_rows, E, D).
+template <typename T>
+static int gatv2_score_grad_run(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const void *f,
+                                int64_t ldf, const float *attn, float slope, const float *ds, float *out, int64_t ldo,
+                                int64_t n_rows, int64_t num_edges, int64_t H, int64_t head_dim, int accumulate,
+                                void *ws, size_t ws_bytes, cudaStream_t stream) {
+    const int64_t D = H * head_dim;
+    const Shape s = pick_shape(D, true);   // the copy-sum kernel of hub pass 2; one tile (D <= 128)
+    const bool need_hub = num_edges > HUB_T;
+    HubWs h{};
+    if (need_hub) {
+        h = layout_ws(ws, num_edges, D);
+        PGLB_CHECK_ARG(ws != nullptr && ws_bytes >= h.bytes, PGLB_EWORKSPACE,
+                       "pglb_gatv2_score_grad: workspace of %zu bytes needed (got %zu)", h.bytes, ws_bytes);
+        PGLB_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
+                       "pglb_gatv2_score_grad: workspace must be 256-byte aligned");
+        PGLB_CUDA(cudaMemsetAsync(h.hub_count, 0, 8, stream));
+    }
+    V2GradP p{};
+    p.rbeg = indptr;
+    p.rend = indptr + 1;
+    p.indptr = indptr;
+    p.n_ind = n_rows;
+    p.cols = cols;
+    p.eid = eid;
+    p.f = f;
+    p.ldf = ldf;
+    p.attn = attn;
+    p.ds = ds;
+    p.slope = slope;
+    p.H = (int)H;
+    p.D = (int)D;
+    p.head_dim = (int)head_dim;
+    p.out = out;
+    p.ldo = ldo;
+    p.n_rows = n_rows;
+    p.accumulate = accumulate;
+    p.hub_threshold = need_hub ? HUB_T : INT64_MAX;
+    p.hub_count = h.hub_count;
+    p.hub_rows = h.hub_rows;
+    const int64_t gpb = kThreads / s.g;
+    auto launch = [&](const V2GradP &q, int64_t blocks) {
+        switch (s.g) {
+            case 4: launch_v2_grad<T, 4>(q, blocks, stream); break;
+            case 8: launch_v2_grad<T, 8>(q, blocks, stream); break;
+            case 16: launch_v2_grad<T, 16>(q, blocks, stream); break;
+            default: launch_v2_grad<T, 32>(q, blocks, stream); break;
+        }
+    };
+    {
+        const int64_t blocks = (n_rows + gpb - 1) / gpb;
+        PGLB_CHECK_ARG(blocks <= 0x7fffffffLL, PGLB_ESHAPE, "pglb_gatv2_score_grad: grid too large");
+        launch(p, blocks);
+        PGLB_LAUNCH_CHECK("gatv2_score_grad_kernel");
+    }
+    if (need_hub) {
+        hub_plan_kernel<<<1, 1024, 0, stream>>>(indptr, h.hub_count, h.hub_rows, h.chunk_off, h.vbeg, h.vend,
+                                                h.total_chunks, h.n_hubs);
+        PGLB_LAUNCH_CHECK("hub_plan_kernel");
+        const int64_t max_blocks = (int64_t)sm_count() * 8;
+        // pass 1: chunk -> fp32 partial
+        V2GradP p1 = p;
+        p1.rbeg = h.vbeg;
+        p1.rend = h.vend;
+        p1.out = h.partial;
+        p1.ldo = h.dpad;
+        p1.n_rows = 0;
+        p1.n_rows_dev = h.total_chunks;
+        p1.chunks = 1;
+        p1.accumulate = 0;
+        p1.hub_threshold = INT64_MAX;
+        {
+            int64_t blocks = (h.chunk_cap + gpb - 1) / gpb;
+            if (blocks > max_blocks) blocks = max_blocks;
+            launch(p1, blocks);
+            PGLB_LAUNCH_CHECK("gatv2_score_grad_kernel(hub pass 1)");
+        }
+        // pass 2: the partials of a hub, in chunk order, into its output row
+        SpmmP p2{};
+        p2.rbeg = h.chunk_off;
+        p2.rend = h.chunk_off + 1;
+        p2.x = h.partial;
+        p2.ldx = h.dpad;
+        p2.out = out;
+        p2.ldo = ldo;
+        p2.n_rows_dev = h.n_hubs;
+        p2.D = (int)D;
+        p2.head_dim = 1;
+        p2.msg_op = PGLB_MSG_COPY;
+        p2.reduce_op = PGLB_REDUCE_SUM;
+        p2.row_map = h.hub_rows;
+        p2.rpg = 1;
+        p2.contig = 0;
+        p2.hub_threshold = INT64_MAX;
+        p2.accumulate = accumulate;
+        {
+            int64_t blocks = (h.hub_cap + gpb - 1) / gpb;
+            if (blocks > max_blocks) blocks = max_blocks;
+            dim3 grid((unsigned)blocks, (unsigned)s.tiles);
+            pick_kernel<float, float>(s, 0, 0)<<<grid, kThreads, 0, stream>>>(p2);
             PGLB_LAUNCH_CHECK("spmm_csr_kernel(hub pass 2)");
         }
     }
@@ -965,6 +1198,92 @@ extern "C" int pglb_dot_attn_drop_csr_x16(const int64_t *indptr, const int64_t *
     return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
 }
 
+// The argument checks and the launch of the GATv2 attention entries (include/pglb.h).  T: element type of f and out.
+// Every check precedes any CUDA call.  drop (nullable): the attention-dropout stream.
+template <typename T>
+static int gatv2_attn_entry(const char *name, const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
+                            const float *attn, float slope, void *out, int64_t ldo, float *lse, int64_t n,
+                            int64_t num_edges, int64_t H, int64_t head_dim, void *ws, size_t ws_bytes, void *stream_,
+                            const AttnDrop *drop) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    constexpr int64_t B = sizeof(T);
+    PGLB_CHECK_ARG(n >= 0 && num_edges >= 0 && H > 0 && head_dim > 0, PGLB_EINVAL, "%s: bad size", name);
+    const int64_t D = H * head_dim;
+    const int64_t lph = head_dim / 4;
+    PGLB_CHECK_ARG(D <= 128 && head_dim % 4 == 0 && (lph & (lph - 1)) == 0 && (D * B) % 16 == 0 &&
+                       num_edges < 0x7fffffffLL && n < 0x7fffffffLL,
+                   PGLB_EUNSUPPORTED, "%s: needs H*head_dim <= 128 in 16-byte rows, head_dim in {4, 8, ..., 128}", name);
+    PGLB_CHECK_ARG(slope >= 0.0f && slope <= 1.0f, PGLB_EUNSUPPORTED, "%s: needs 0 <= negative_slope <= 1", name);
+    PGLB_CHECK_ARG(!drop || H % 4 == 0, PGLB_EUNSUPPORTED, "%s: attention dropout needs H %% 4 == 0", name);
+    if (n == 0) return PGLB_OK;
+    PGLB_CHECK_ARG(indptr && out, PGLB_EINVAL, "%s: NULL pointer", name);
+    PGLB_CHECK_ARG(ldf >= D && ldo >= D && (ldo * B) % 16 == 0 && aligned16(out) &&
+                       (num_edges == 0 || gatv2_attn_takes<T>(D, head_dim, slope, f, ldf, attn, n)),
+                   PGLB_ESHAPE, "%s: rows must be 16-byte aligned", name);
+    if (num_edges == 0) {
+        PGLB_CUDA(cudaMemset2DAsync(out, B * ldo, 0, B * D, n, stream));
+        return PGLB_OK;
+    }
+    PGLB_CHECK_ARG(cols && f && attn, PGLB_EINVAL, "%s: NULL pointer", name);
+    PGLB_CHECK_ARG(ws && (reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
+                   "%s: workspace NULL or not 256-byte aligned", name);
+    return gatv2_attn_run<T>(indptr, cols, f, ldf, attn, slope, out, ldo, lse, n, num_edges, H, head_dim, drop, ws,
+                             ws_bytes, stream);
+}
+
+extern "C" int pglb_gatv2_attn_csr_f32(const int64_t *indptr, const int64_t *cols, const float *f, int64_t ldf,
+                                       const float *attn, float negative_slope, float *out, int64_t ldo, float *lse,
+                                       int64_t n, int64_t num_edges, int64_t H, int64_t head_dim, void *ws,
+                                       size_t ws_bytes, void *stream_) {
+    return gatv2_attn_entry<float>("pglb_gatv2_attn_csr_f32", indptr, cols, f, ldf, attn, negative_slope, out, ldo, lse,
+                                   n, num_edges, H, head_dim, ws, ws_bytes, stream_, nullptr);
+}
+
+extern "C" int pglb_gatv2_attn_csr_x16(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
+                                       const float *attn, float negative_slope, void *out, int64_t ldo, float *lse,
+                                       int64_t n, int64_t num_edges, int64_t H, int64_t head_dim, int dtype, void *ws,
+                                       size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_gatv2_attn_csr_x16";
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    auto run = [&](auto *elem) -> int {
+        using T = std::remove_pointer_t<decltype(elem)>;
+        return gatv2_attn_entry<T>(name, indptr, cols, f, ldf, attn, negative_slope, out, ldo, lse, n, num_edges, H,
+                                   head_dim, ws, ws_bytes, stream_, nullptr);
+    };
+    return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
+}
+
+extern "C" int pglb_gatv2_attn_drop_csr_f32(const int64_t *indptr, const int64_t *cols, const float *f, int64_t ldf,
+                                            const float *attn, float negative_slope, float *out, int64_t ldo,
+                                            float *lse, int64_t n, int64_t num_edges, int64_t H, int64_t head_dim,
+                                            float attn_drop, uint64_t seed, uint64_t offset, void *ws, size_t ws_bytes,
+                                            void *stream_) {
+    const char *name = "pglb_gatv2_attn_drop_csr_f32";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    return gatv2_attn_entry<float>(name, indptr, cols, f, ldf, attn, negative_slope, out, ldo, lse, n, num_edges, H,
+                                   head_dim, ws, ws_bytes, stream_, &drop);
+}
+
+extern "C" int pglb_gatv2_attn_drop_csr_x16(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
+                                            const float *attn, float negative_slope, void *out, int64_t ldo,
+                                            float *lse, int64_t n, int64_t num_edges, int64_t H, int64_t head_dim,
+                                            int dtype, float attn_drop, uint64_t seed, uint64_t offset, void *ws,
+                                            size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_gatv2_attn_drop_csr_x16";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    auto run = [&](auto *elem) -> int {
+        using T = std::remove_pointer_t<decltype(elem)>;
+        return gatv2_attn_entry<T>(name, indptr, cols, f, ldf, attn, negative_slope, out, ldo, lse, n, num_edges, H,
+                                   head_dim, ws, ws_bytes, stream_, &drop);
+    };
+    return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
+}
+
 // Send/recv with an edge operand over 16-bit x / out (include/pglb.h): the node-parallel kernel with MODE 1 -- the
 // reverse-CSR aggregation of the fused GAT backward (grad f = sum over out-edges of alpha * grad_out[dst]).
 extern "C" int pglb_spmm_csr_ue_x16(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const void *x,
@@ -1007,4 +1326,56 @@ extern "C" int pglb_spmm_csr_ue_x16(const int64_t *indptr, const int64_t *cols, 
                                    ws_bytes, stream);
     };
     return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
+}
+
+// The checks and the launch of the GATv2 score-gradient entries (include/pglb.h).  T: element type of f.
+template <typename T>
+static int gatv2_score_grad_entry(const char *name, const int64_t *indptr, const int64_t *cols, const int64_t *eid,
+                                  const void *f, int64_t ldf, const float *attn, float slope, const float *ds,
+                                  float *out, int64_t ldo, int64_t n_rows, int64_t num_edges, int64_t H,
+                                  int64_t head_dim, int accumulate, void *ws, size_t ws_bytes, void *stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    constexpr int64_t B = sizeof(T);
+    PGLB_CHECK_ARG(n_rows >= 0 && num_edges >= 0 && H > 0 && head_dim > 0, PGLB_EINVAL, "%s: bad size", name);
+    const int64_t D = H * head_dim;
+    PGLB_CHECK_ARG(D <= 128 && head_dim % 4 == 0 && (D * B) % 16 == 0, PGLB_EUNSUPPORTED,
+                   "%s: needs H*head_dim <= 128 in 16-byte rows and head_dim %% 4 == 0", name);
+    PGLB_CHECK_ARG(slope >= 0.0f && slope <= 1.0f, PGLB_EUNSUPPORTED, "%s: needs 0 <= negative_slope <= 1", name);
+    if (n_rows == 0) return PGLB_OK;
+    PGLB_CHECK_ARG(indptr && out && (num_edges == 0 || (cols && f && attn && ds)), PGLB_EINVAL, "%s: NULL pointer",
+                   name);
+    PGLB_CHECK_ARG(ldf >= D && ldo >= D && (ldf * B) % 16 == 0 && ldo % 4 == 0 && aligned16(f) && aligned16(out) &&
+                       aligned16(attn),
+                   PGLB_ESHAPE, "%s: rows must be 16-byte aligned", name);
+    if (num_edges == 0) {
+        if (!accumulate) PGLB_CUDA(cudaMemset2DAsync(out, 4 * ldo, 0, 4 * D, n_rows, stream));
+        return PGLB_OK;
+    }
+    return gatv2_score_grad_run<T>(indptr, cols, eid, f, ldf, attn, slope, ds, out, ldo, n_rows, num_edges, H,
+                                   head_dim, accumulate, ws, ws_bytes, stream);
+}
+
+extern "C" int pglb_gatv2_score_grad_f32(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const float *f,
+                                         int64_t ldf, const float *attn, float negative_slope, const float *ds,
+                                         float *out, int64_t ldo, int64_t n_rows, int64_t num_edges, int64_t H,
+                                         int64_t head_dim, int accumulate, void *ws, size_t ws_bytes, void *stream_) {
+    return gatv2_score_grad_entry<float>("pglb_gatv2_score_grad_f32", indptr, cols, eid, f, ldf, attn, negative_slope,
+                                         ds, out, ldo, n_rows, num_edges, H, head_dim, accumulate, ws, ws_bytes,
+                                         stream_);
+}
+
+extern "C" int pglb_gatv2_score_grad_x16(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const void *f,
+                                         int64_t ldf, const float *attn, float negative_slope, const float *ds,
+                                         float *out, int64_t ldo, int64_t n_rows, int64_t num_edges, int64_t H,
+                                         int64_t head_dim, int dtype, int accumulate, void *ws, size_t ws_bytes,
+                                         void *stream_) {
+    const char *name = "pglb_gatv2_score_grad_x16";
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    if (dtype == PGLB_DTYPE_BF16)
+        return gatv2_score_grad_entry<__nv_bfloat16>(name, indptr, cols, eid, f, ldf, attn, negative_slope, ds, out,
+                                                     ldo, n_rows, num_edges, H, head_dim, accumulate, ws, ws_bytes,
+                                                     stream_);
+    return gatv2_score_grad_entry<__half>(name, indptr, cols, eid, f, ldf, attn, negative_slope, ds, out, ldo, n_rows,
+                                          num_edges, H, head_dim, accumulate, ws, ws_bytes, stream_);
 }

@@ -1054,7 +1054,45 @@ int spmm_v5_run(const int64_t *indptr, const int64_t *cols, const void *x, int64
     return launch_v5<T>(p, cols32 != nullptr && cols != nullptr && l2_hints != 0, stream);
 }
 
+template <typename T>
+bool gatv2_attn_takes(int64_t D, int64_t head_dim, float slope, const void *f, int64_t ldf, const float *attn,
+                      int64_t n_src) {
+    return gatv2_attn_eligible<T>(D, head_dim, slope, f, ldf, attn, n_src);
+}
+
+// Single-pass GATv2 attention (GATv2Conv): out[d,h,:] = sum_j softmax_j(sum_c a[h,c] lrelu(f[src_j,h,c] + f[d,h,c]))
+// f[src_j,h,:] on spmm_gat5_kernel<kScoreV2>.  T: element type of f and out; the call is one gatv2_attn_takes accepts.
+// attn: a [H * head_dim] float32.  lse (nullable): the rows' log-sum-exp.  drop (nullable): the attention-dropout stream.
+template <typename T>
+int gatv2_attn_run(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf, const float *attn,
+                   float slope, void *out, int64_t ldo, float *lse, int64_t n, int64_t E, int64_t H, int64_t head_dim,
+                   const AttnDrop *drop, void *ws, size_t ws_bytes, cudaStream_t stream) {
+    StreamP p{};
+    p.ldy = H;
+    p.head_dim = (int)head_dim;
+    p.slope = slope;
+    p.lse = lse;
+    {
+        const int rc = stream_prepare(p, gat_task_size(E), indptr, cols, f, ldf, out, ldo, n, E, H * head_dim,
+                                      PGLB_REDUCE_SUM, nullptr, nullptr, nullptr, nullptr, ws, ws_bytes, stream);
+        if (rc) return rc;
+    }
+    p.dyn = dyn_mode("PGLB_GAT_DYN", 1, p.ntasks);
+    {
+        const int rc = launch_empty_rows<T>(p, stream);
+        if (rc) return rc;
+    }
+    if (drop) return launch_gatv2_attn<T, true>(p, attn, *drop, stream);
+    return launch_gatv2_attn<T, false>(p, attn, AttnDrop{}, stream);
+}
+
 // the instantiations the entries in spmm.cu call
+template decltype(gatv2_attn_takes<float>) gatv2_attn_takes<float>;
+template decltype(gatv2_attn_takes<__nv_bfloat16>) gatv2_attn_takes<__nv_bfloat16>;
+template decltype(gatv2_attn_takes<__half>) gatv2_attn_takes<__half>;
+template decltype(gatv2_attn_run<float>) gatv2_attn_run<float>;
+template decltype(gatv2_attn_run<__nv_bfloat16>) gatv2_attn_run<__nv_bfloat16>;
+template decltype(gatv2_attn_run<__half>) gatv2_attn_run<__half>;
 template decltype(v5_eligible<float>) v5_eligible<float>;
 template decltype(v5_eligible<__nv_bfloat16>) v5_eligible<__nv_bfloat16>;
 template decltype(v5_eligible<__half>) v5_eligible<__half>;

@@ -271,7 +271,9 @@ class PinSageConv(nn.Module):
 
 
 class GATv2Conv(nn.Module):
-    """reference pgl/nn/conv.py:349-435."""
+    """reference pgl/nn/conv.py:349-435.  On a ``Graph`` the attention (send_uv(add), LeakyReLU, the sum with attn,
+    edge_softmax, dropout, send_ue_recv) is one fused pass with a fused backward (``ops.gatv2_attention``); shapes
+    those kernels refuse keep the op-by-op route."""
 
     def __init__(self, input_size, hidden_size, feat_drop=0.6, attn_drop=0.6, num_heads=1,
                  concat=True, activation=None):
@@ -294,14 +296,23 @@ class GATv2Conv(nn.Module):
         if self.feat_drop > 1e-15:
             feature = self.feat_dropout(feature)
         feature = self.linear(feature).reshape(-1, self.num_heads, self.hidden_size)
-        alpha = graph.send_uv(feature, feature, "add")
-        alpha = self.leaky_relu(alpha)
-        alpha = torch.sum(alpha * self.attn, dim=-1)
-        alpha = GF.edge_softmax(graph, alpha)
-        alpha = alpha.reshape(-1, self.num_heads, 1)
-        if self.attn_drop > 1e-15:
-            alpha = self.attn_dropout(alpha)
-        output = graph.send_ue_recv(feature, alpha, "mul", "sum")
+        output = None
+        if type(graph).__name__ == "Graph" and feature.is_cuda:
+            # score, softmax, dropout and weighted sum in one pass with a fused backward (ops._GatV2): no [E, H*Dh]
+            # tensor; None when the call is outside the kernels
+            from .. import ops
+            drop = self.attn_drop if self.attn_drop > 1e-15 and self.training else 0.0
+            output = ops.gatv2_attention(graph._fwd_csr(), graph._bwd_csr, feature, self.attn,
+                                         self.leaky_relu.negative_slope, attn_drop=drop)
+        if output is None:
+            alpha = graph.send_uv(feature, feature, "add")
+            alpha = self.leaky_relu(alpha)
+            alpha = torch.sum(alpha * self.attn, dim=-1)
+            alpha = GF.edge_softmax(graph, alpha)
+            alpha = alpha.reshape(-1, self.num_heads, 1)
+            if self.attn_drop > 1e-15:
+                alpha = self.attn_dropout(alpha)
+            output = graph.send_ue_recv(feature, alpha, "mul", "sum")
         if self.concat:
             output = output.reshape(-1, self.num_heads * self.hidden_size)
         else:

@@ -1813,6 +1813,134 @@ def dot_attention(fwd, bwd, q, k, v, attn_drop=0.0, seed=None):
     return out.reshape(n, H, Dh)
 
 
+def _gatv2_fwd_raw(fwd, f2, a32, slope, H, Dh, drop, want_lse):
+    """pglb_gatv2_attn_* on [N, H*Dh] rows: (out in f2's dtype, lse or None)."""
+    n = int(f2.shape[0])
+    E = int(fwd["cols"].shape[0])
+    out = torch.empty((n, H * Dh), dtype=f2.dtype, device=f2.device)
+    lse = torch.zeros((n, H), dtype=torch.float32, device=f2.device) if want_lse else None
+    need = ctypes.c_size_t(0)
+    check(lib.pglb_spmm_csr_ws(n, E, H * Dh, ctypes.byref(need)))
+    ws = workspace(f2.device, need.value)
+    args = (_ptr(fwd["indptr"]), _ptr(fwd["cols"]), _ptr(f2), f2.stride(0), _ptr(a32), float(slope), _ptr(out),
+            out.stride(0), _ptr(lse), n, E, H, Dh)
+    dt = (_DTYPE16[f2.dtype],) if f2.dtype in HALF_DTYPES else ()
+    fn = {(False, False): lib.pglb_gatv2_attn_csr_f32, (False, True): lib.pglb_gatv2_attn_csr_x16,
+          (True, False): lib.pglb_gatv2_attn_drop_csr_f32, (True, True): lib.pglb_gatv2_attn_drop_csr_x16}
+    with torch.cuda.device(f2.device):
+        check(fn[(drop is not None, bool(dt))](*args, *dt, *(drop or ()), _ptr(ws), ws.numel(), _stream()))
+    return out, lse
+
+
+class _GatV2(torch.autograd.Function):
+    """GATv2Conv's attention under autograd (reference pgl/nn/conv.py:420-427 differentiated by Paddle over send_uv(add),
+    LeakyReLU, the product with attn, a sum, edge_softmax, dropout and send_ue_recv).  Forward = pglb_gatv2_attn_* (one
+    pass; keeps only lse[N, H]).  Backward = one edge kernel (pglb_gatv2_bwd_edge_*: scores and weights rebuilt, beta,
+    ds and grad attn) + the score-gradient aggregation on the dst-keyed and the src-keyed CSR (pglb_gatv2_score_grad_*:
+    the [E, H*Dh] dz is recomputed, never stored) + send_ue_recv(G, beta) on the src-keyed CSR.  16-bit f2 takes the
+    *_x16 entries: lse, beta, ds, the score terms and a32 are float32, grad f comes back in f2's dtype.
+    drop = (p, seed, offset): attention dropout recomputed from (seed, offset) in the forward and the backward."""
+
+    @staticmethod
+    def forward(ctx, f2, a32, fwd, bwd, slope, H, Dh, drop):
+        out, lse = _gatv2_fwd_raw(fwd, f2, a32, slope, H, Dh, drop, True)
+        ctx.meta = (fwd, bwd, slope, H, Dh, drop)
+        ctx.save_for_backward(f2, a32, out, lse)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        fwd, bwd, slope, H, Dh, drop = ctx.meta
+        bwd = bwd() if callable(bwd) else bwd
+        f2, a32, out, lse = ctx.saved_tensors
+        half = f2.dtype in HALF_DTYPES
+        g = _f32_2d(g.to(f2.dtype) if g.dtype != f2.dtype else g, allow16=half)
+        E = int(fwd["cols"].shape[0])
+        n, D = int(f2.shape[0]), H * Dh
+        dev = g.device
+        beta = torch.empty((E, H), dtype=torch.float32, device=dev)
+        ds = torch.empty((E, H), dtype=torch.float32, device=dev)
+        ga = torch.empty((D,), dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
+        need_e, need_a = ctypes.c_size_t(0), ctypes.c_size_t(0)
+        check(lib.pglb_gatv2_bwd_edge_ws(E, ctypes.byref(need_e)))
+        check(lib.pglb_spmm_csr_ws(n, E, D, ctypes.byref(need_a)))
+        ws = workspace(dev, max(need_e.value, need_a.value))
+        dt = (_DTYPE16[f2.dtype],) if half else ()
+        fn = {(False, False): lib.pglb_gatv2_bwd_edge_f32, (False, True): lib.pglb_gatv2_bwd_edge_x16,
+              (True, False): lib.pglb_gatv2_bwd_edge_drop_f32, (True, True): lib.pglb_gatv2_bwd_edge_drop_x16}
+        gf = None
+        with torch.cuda.device(dev):
+            check(fn[(drop is not None, half)](
+                _ptr(fwd["rows"]), _ptr(fwd["cols"]), _ptr(fwd["eid"]), _ptr(f2), f2.stride(0), _ptr(a32), float(slope),
+                _ptr(g), g.stride(0), _ptr(out), out.stride(0), _ptr(lse), E, H, Dh, *dt, *(drop or ()), _ptr(beta),
+                _ptr(ds), _ptr(ga), _ptr(ws), ws.numel(), _stream()))
+            if ctx.needs_input_grad[0]:
+                # grad f = the dst term (dst-keyed CSR) + the src term (src-keyed CSR) + sum over out-edges of beta G[dst]
+                gr = torch.empty((n, D), dtype=torch.float32, device=dev)
+                score = lib.pglb_gatv2_score_grad_x16 if half else lib.pglb_gatv2_score_grad_f32
+                for csr, acc in ((fwd, 0), (bwd, 1)):
+                    check(score(_ptr(csr["indptr"]), _ptr(csr["cols"]), _ptr(csr["eid"]), _ptr(f2), f2.stride(0),
+                                _ptr(a32), float(slope), _ptr(ds), _ptr(gr), gr.stride(0), n, E, H, Dh, *dt, acc,
+                                _ptr(ws), ws.numel(), _stream()))
+                gv = _spmm_raw(bwd["indptr"], bwd["cols"], g, n, "sum", eid=bwd["eid"], y2=beta, y_bcast=BCAST_HEAD,
+                               head_dim=Dh, msg_op="mul", max_degree=bwd.get("max_degree", -1))
+                gf = gr.add_(gv.float() if half else gv)
+                gf = gf.to(f2.dtype) if half else gf
+        return gf, ga, None, None, None, None, None, None
+
+
+def gatv2_attention(fwd, bwd, f, attn, negative_slope, out_dtype=None, attn_drop=0.0, seed=None):
+    """GATv2Conv's attention in one pass:
+    out[d,h,:] = sum over the in-edges j of d of softmax_j(sum_c attn[h,c] lrelu(f[src_j,h,c] + f[d,h,c])) f[src_j,h,:]
+    with a fused backward when autograd needs one.  f [N, H, Dh] on one graph (n_dst == N), attn [H, Dh] or
+    [1, H, Dh]; ``fwd`` is the dst-keyed CSR dict (with ``rows``), ``bwd`` the src-keyed one or a callable returning
+    it.  The result dtype is ``out_dtype``, or by default torch's promotion of f's and attn's dtypes.  float32 f runs the
+    float32 kernels (attn widened to float32); bfloat16 / float16 f runs the 16-bit kernels when the result dtype is f's
+    (attn widened to float32, grad f in f's dtype, grad attn in attn's dtype).  Returns [N, H, Dh], or None when the
+    call is outside the kernels (float64, another dtype mix, H*Dh > 128, Dh not a power of two >= 4, slope outside
+    [0, 1], rows the kernels cannot read, n_dst != N, no edges, attn_drop >= 1, dropout with H % 4 != 0 or during
+    CUDA-graph capture); the caller then keeps the op-by-op path.
+    ``attn_drop`` in (0, 1): dropout on the normalised attention per edge and head inside the kernels, the mask drawn
+    from ``seed`` = (seed, offset), offset a multiple of 4, or by default from the default CUDA generator of f's device
+    (whose offset then advances by 4), as GATConv's fused path does."""
+    require_cuda(f, attn)
+    if f.dim() != 3:
+        return None
+    n, H, Dh = (int(s) for s in f.shape)
+    if attn.numel() != H * Dh or attn.shape[-2:] != (H, Dh):
+        return None
+    half = f.dtype in HALF_DTYPES
+    res = _result_dtype(out_dtype, f, attn)
+    if torch.float64 in (f.dtype, attn.dtype) or not (f.dtype == torch.float32 or (half and res == f.dtype)):
+        return None
+    if H * Dh > 128 or Dh < 4 or Dh & (Dh - 1) or (H * Dh * f.element_size()) % 16:
+        return None
+    slope = float(negative_slope)
+    if not 0.0 <= slope <= 1.0:
+        return None
+    attn_drop = float(attn_drop)
+    if not 0.0 <= attn_drop < 1.0 or (attn_drop > 0.0 and H % 4):
+        return None
+    if attn_drop > 0.0 and torch.cuda.is_current_stream_capturing():
+        return None     # the generator's offset advances on the host: not replayable by a graph
+    if int(fwd["indptr"].shape[0]) - 1 != n or int(fwd["cols"].shape[0]) == 0 or fwd.get("rows") is None:
+        return None
+    f2 = _f32_2d(f, allow16=half)
+    a32 = attn.reshape(H * Dh)
+    a32 = (a32.float() if a32.dtype != torch.float32 else a32).contiguous()
+    if f2.data_ptr() % 16 or (f2.stride(0) * f2.element_size()) % 16 or a32.data_ptr() % 16:
+        return None
+    drop = None
+    if attn_drop > 0.0:
+        drop = (attn_drop,) + (tuple(int(s) for s in seed) if seed is not None else _attn_drop_stream(f2.device))
+    if torch.is_grad_enabled() and (f.requires_grad or attn.requires_grad):
+        out = _GatV2.apply(f2, a32, fwd, bwd, slope, H, Dh, drop)
+    else:
+        out = _gatv2_fwd_raw(fwd, f2, a32, slope, H, Dh, drop, False)[0]
+    out = out.reshape(n, H, Dh)
+    return out if out.dtype == res else out.to(res)
+
+
 @f64_through
 def aggregate_ue_slots(x, y_slots, fwd, n_dst, message_op="mul", reduce_op="sum"):
     """send_ue_recv whose edge operand is already in CSR slot order (read sequentially)."""
