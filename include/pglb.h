@@ -559,6 +559,38 @@ int pglb_linear_tf32x3_f32(const float *x, int64_t ldx, const float *w, const fl
                            int64_t ldo, int64_t M, int64_t K, int64_t N, int act, void *stream);
 
 /* ------------------------------------------------------------------------------------
+ * RGCNConv's relation-typed aggregation (pgl/nn/conv.py:998-1024: sum_r send_recv(x @ W_r, mean) over the
+ * relations' graphs), reassociated as out[d] = sum_r A_r[d] W_r with A_r[d] the mean of x[src] over the r-run of
+ * row d.  The CSR is typed: the slots of every row are grouped by relation, ascending relation id, so a row's r-run
+ * is one contiguous slot range; rel[slot] is its relation (int16).  fp32 only, 3xTF32 products with fp32
+ * accumulation (the accuracy contract of pglb_linear_tf32x3_f32).  No floating-point atomics: outputs are
+ * bit-identical run to run.  Every argument check returns PGLB_EINVAL before any CUDA call.
+ * ---------------------------------------------------------------------------------- */
+
+/* out[n_rows, N] (row stride ldo): out[d] = sum_r A_r[d] weight[r], weight contiguous [num_rels, K, N].
+ * slot_w NULL: A_r[d] = mean over the r-run of x[cols[j]] (0 for an empty run) -- the forward on the typed dst-CSR.
+ * slot_w non-NULL: A_r[d] = sum over the r-run of slot_w[j] x[cols[j]] -- grad x on the typed src-CSR with
+ * slot_w[j] = 1 / cnt_r(dst_j) and weight = W^T [num_rels, O, D].  K, N multiples of 4 in [4, 128]; x 16-byte and
+ * out 8-byte aligned, ldx % 4 == 0, ldo even; relation ids in [0, num_rels), num_rels <= 32767. */
+int pglb_rgcn_agg_f32(const int64_t *indptr, const int64_t *cols, const int16_t *rel, const float *slot_w,
+                      const float *x, int64_t ldx, const float *weight, int64_t num_rels, int64_t K, int64_t N,
+                      float *out, int64_t ldo, int64_t n_rows, void *stream);
+
+/* grad_weight[num_rels, D, O] = sum over the runs p of relation r of A_p^T grad_out[run_row[p]], A_p the mean of
+ * x[cols[j]] over slots [run_beg[p], run_end[p]) of the typed dst-CSR.  The runs are sorted by relation: relation r
+ * owns runs [run_off[r], run_off[r + 1]).  Work item i of relation r covers runs run_off[r] + (i - item_off[r]) * chunk
+ * onward (chunk runs at most); item_off[num_rels + 1] is ascending with item_off[num_rels] = n_items.  Each item writes
+ * an fp32 [D, O] partial into ws (pglb_rgcn_wgrad_ws bytes, 16-byte aligned), and a second launch adds a relation's
+ * partials in item order (a relation without runs gets 0).  D, O multiples of 4 in [4, 128]; x and grad_out 16-byte
+ * aligned with ldx, ldg multiples of 4. */
+int pglb_rgcn_wgrad_ws(int64_t n_items, int64_t D, int64_t O, size_t *ws_bytes);
+int pglb_rgcn_wgrad_f32(const int64_t *run_row, const int64_t *run_beg, const int64_t *run_end,
+                        const int64_t *run_off, const int64_t *item_off, int64_t num_rels, int64_t n_items,
+                        int64_t chunk, const int64_t *cols, const float *x, int64_t ldx, const float *grad_out,
+                        int64_t ldg, int64_t D, int64_t O, float *grad_weight, void *ws, size_t ws_bytes,
+                        void *stream);
+
+/* ------------------------------------------------------------------------------------
  * Neighbour sampling + reindex for mini-batch GraphSAGE (SURVEY 8f rank 4).  Replace
  * paddle.geometric.sample_neighbors / reindex_graph as called by NeighborSampler.sample_neighbors
  * (pgl/sampling/sage.py:130-155) on the cached dst-CSR (row = adj_dst_index._sorted_v,

@@ -7,8 +7,9 @@ CUDA tensors as the device container and hand-written CUDA kernels behind a C-AB
 (include/pglb.h, libpglb.so).  Importing this package fails if libpglb.so has not been built.
 """
 from . import _lib  # noqa: F401  (raises ImportError when the native library is missing)
-from . import bigraph, graph, math, message, nn, ops, partition, sampling, utils  # noqa: F401
+from . import bigraph, graph, heter_graph, math, message, nn, ops, partition, sampling, utils  # noqa: F401
 from .bigraph import BiGraph  # noqa: F401
 from .graph import DistGPUGraph, Graph  # noqa: F401
+from .heter_graph import HeterGraph  # noqa: F401
 
 __version__ = "0.1.0"

@@ -156,7 +156,11 @@ _SIGS = {
                                           _i64, c_int, _p, c_size_t, _p]),
     "pglb_gatv2_score_grad_x16": (c_int, [_p, _p, _p, _p, _i64, _p, ctypes.c_float, _p, _p, _i64, _i64, _i64, _i64,
                                           _i64, c_int, c_int, _p, c_size_t, _p]),
-    "pglb_gat_attention_csr_f32": (c_int, [_p, _p, _p, _p, ctypes.c_float, _p, _i64, _i64, _i64, _p,
+    "pglb_rgcn_agg_f32": (c_int, [_p, _p, _p, _p, _p, _i64, _p, _i64, _i64, _i64, _p, _i64, _i64, _p]),
+    "pglb_rgcn_wgrad_ws": (c_int, [_i64, _i64, _i64, POINTER(c_size_t)]),
+    "pglb_rgcn_wgrad_f32": (c_int, [_p, _p, _p, _p, _p, _i64, _i64, _i64, _p, _p, _i64, _p, _i64, _i64, _i64, _p, _p,
+                                    c_size_t, _p]),
+    "pglb_gat_attention_csr_f32":(c_int, [_p, _p, _p, _p, ctypes.c_float, _p, _i64, _i64, _i64, _p,
                                            c_size_t, _p]),
     "pglb_sddmm_dot_f32": (c_int, [_p, _p, _p, _i64, _p, _i64, _i64, _i64, _i64, _p, _p]),
     "pglb_edge_softmax_bwd_csr_f32": (c_int, [_p, _p, _p, _p, _p, _i64, _i64, _i64, _p]),

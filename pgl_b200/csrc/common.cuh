@@ -88,6 +88,22 @@ int radix_sort_u64(uint64_t *keys, uint64_t *vals, uint64_t *keys_alt, uint64_t 
 __device__ __forceinline__ int64_t ld_stream(const int64_t *p) { return __ldcs((const long long *)p); }
 __device__ __forceinline__ int64_t ld_ro(const int64_t *p) { return __ldg((const long long *)p); }
 
+// 3xTF32 products (linear_tc.cu, rgcn.cu): x*w ~= x_lo*w_hi + x_hi*w_lo + x_hi*w_hi with x_hi = tf32(x),
+// x_lo = tf32(x - x_hi), each term one mma.sync.m16n8k8 accumulating in fp32
+__device__ __forceinline__ uint32_t to_tf32(float v) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
+    return r;
+}
+
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile(
+        "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
+        "{%0,%1,%2,%3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
 // 16-bit feature elements of pglb_spmm_csr_x16, handled as raw bits: widen() is exact, round() is the one
 // round-to-nearest-even of a value computed in fp32.  lo / hi = the element in the low / high half of a 32-bit word.
 template <typename T>

@@ -23,20 +23,6 @@ constexpr int LT_WARPS_DEFAULT = 8;  // 8 warps = 4 row blocks x 2 column groups
 constexpr int LT_KMAX = 128;
 constexpr int LT_XS = LT_KMAX + 4;  // x tile row stride (floats): 132 = 4 mod 32 -> conflict-free A loads
 
-__device__ __forceinline__ uint32_t to_tf32(float v) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
-    return r;
-}
-
-__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
-        "{%0,%1,%2,%3};"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
 __device__ __forceinline__ void cp_async16_zfill(void *smem, const void *gmem, int src_bytes) {
     const uint32_t s = (uint32_t)__cvta_generic_to_shared(smem);
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(s), "l"(gmem), "r"(src_bytes)

@@ -13,6 +13,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from .. import ops
+from ..heter_graph import HeterGraph
 from . import functional as GF
 
 __all__ = ["GCNConv", "GATConv", "GraphSageConv", "Linear", "PinSageConv", "GATv2Conv", "APPNP",
@@ -555,7 +557,10 @@ class GINConv(nn.Module):
 
 class RGCNConv(nn.Module):
     """reference pgl/nn/conv.py:961-1024.  ``graph[etype]`` must give the homogeneous Graph of
-    that relation (a HeterGraph in the reference; any mapping of Graphs here)."""
+    that relation (a HeterGraph in the reference; any mapping of Graphs here).  On a tensor-mode
+    ``HeterGraph`` the layer runs as one relation-typed aggregation (``ops.rgcn_aggregate``) over the
+    graph's typed CSR of ``etypes``; every other input, and every call that path declines, keeps the
+    reference's per-relation loop."""
 
     def __init__(self, in_dim, out_dim, etypes, num_bases=0):
         super().__init__()
@@ -577,6 +582,11 @@ class RGCNConv(nn.Module):
             weight = torch.einsum("rb,bio->rio", self.w_comp, self.weight)
         else:
             weight = self.weight
+        if isinstance(graph, HeterGraph) and graph.is_tensor() and isinstance(feat, torch.Tensor) and feat.is_cuda:
+            fwd, bwd = graph.typed_csr(self.etypes, feat.device)
+            out = ops.rgcn_aggregate(fwd, bwd, feat, weight)
+            if out is not None:
+                return out
         out = None
         for idx, etype in enumerate(self.etypes):
             h = graph[etype].send_recv(feat @ weight[idx], reduce_func="mean")
