@@ -607,6 +607,25 @@ int pglb_sample_count(const int64_t *indptr, const int64_t *nodes, int64_t n, in
 int pglb_sample_fill(const int64_t *indptr, const int64_t *row, const int64_t *eid, const int64_t *nodes,
                      int64_t n, int64_t sample_size, uint64_t seed, const int64_t *offsets,
                      int64_t *out_neighbors, int64_t *out_eids, void *stream);
+/* Relation-typed sampling for HeteroNeighborSampler on a typed in-CSR: indptr / cols (src) / rel (int16 relation of
+ * every slot) with the slots of every row grouped by relation in ascending relation id (heter_graph.typed_in_csr).
+ * sample_sizes: HOST array of num_rels fan-outs k_r (negative = all neighbours, 0 = none, at most 4096), checked on
+ * the host and copied to sizes_dev (device scratch of num_rels int32) on the stream; num_rels in [1, 32767].
+ * Relation r's run of a row is found by binary search over rel: a row costs O(R log deg + sum k_r) however long
+ * it is.  Relation ids outside [0, num_rels) are never sampled.
+ * count[i] = sum_r min(deg_r(nodes[i]), k_r); offsets[0..n] = exclusive scan, offsets[n] = total. */
+int pglb_sample_typed_count(const int64_t *indptr, const int16_t *rel, int64_t num_rels, const int64_t *sample_sizes,
+                            int32_t *sizes_dev, const int64_t *nodes, int64_t n, int64_t *count, int64_t *offsets,
+                            void *stream);
+/* From out_neighbors[offsets[i]] on: the sampled in-neighbours of nodes[i], relation by relation in ascending order;
+ * relation r's run whole in CSR order when deg_r <= k_r or k_r < 0, else a uniform k_r-subset without replacement
+ * (Floyd) whose draw c is mix64(base(seed, i) + r 2^32 + c) -- with one relation, pglb_sample_fill's draws and
+ * output.  out_rel receives the relation of every sampled slot; out_eids (may be NULL) eid[slot] (or the slot when
+ * eid is NULL).  Degrees < 2^31. */
+int pglb_sample_typed_fill(const int64_t *indptr, const int64_t *cols, const int16_t *rel, const int64_t *eid,
+                           int64_t num_rels, const int64_t *sample_sizes, int32_t *sizes_dev, const int64_t *nodes,
+                           int64_t n, uint64_t seed, const int64_t *offsets, int64_t *out_neighbors,
+                           int16_t *out_rel, int64_t *out_eids, void *stream);
 /* Dense lookup table for pglb_reindex_graph: num_nodes int64, filled with INT64_MAX ("empty"). */
 int pglb_reindex_table_init(int64_t *table, int64_t num_nodes, void *stream);
 int pglb_reindex_graph_ws(int64_t num_neighbors, size_t *ws_bytes);

@@ -75,6 +75,8 @@ _SIGS = {
     "pglb_degree_norm_f32": (c_int, [_p, _i64, _p, _p]),
     "pglb_sample_count": (c_int, [_p, _p, _i64, _i64, _p, _p, _p]),
     "pglb_sample_fill": (c_int, [_p, _p, _p, _p, _i64, _i64, ctypes.c_uint64, _p, _p, _p, _p]),
+    "pglb_sample_typed_count": (c_int, [_p, _p, _i64, _p, _p, _p, _i64, _p, _p, _p]),
+    "pglb_sample_typed_fill": (c_int, [_p, _p, _p, _p, _i64, _p, _p, _p, _i64, ctypes.c_uint64, _p, _p, _p, _p, _p]),
     "pglb_reindex_table_init": (c_int, [_p, _i64, _p]),
     "pglb_reindex_graph_ws": (c_int, [_i64, POINTER(c_size_t)]),
     "pglb_reindex_graph": (c_int, [_p, _i64, _p, _p, _i64, _p, _p, _p, _p, _p, _p, c_size_t, _p]),

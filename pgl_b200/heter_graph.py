@@ -236,10 +236,25 @@ class HeterGraph(object):
         return cache[key]
 
 
+def typed_in_csr(edge_lists, num_nodes):
+    """The dst-keyed CSR of all relations together: the edges of ``edge_lists[r]`` ([E_r, 2] int64 CUDA tensors,
+    (src, dst) rows) concatenated in order and run through the stable ``ops.csr_build``, so the slots of every row
+    come out grouped by relation in ascending relation id, ascending eid inside a group.  Returns a dict: indptr,
+    cols (src), rows (dst), eid (index into the concatenation), rel (int16 relation per slot), and per edge of the
+    concatenation src, dst, rel_e.  The typed sampler (sampling.sample_typed_neighbors) reads indptr / cols / rel."""
+    dev = edge_lists[0].device
+    src = torch.cat([e.reshape(-1, 2)[:, 0] for e in edge_lists])
+    dst = torch.cat([e.reshape(-1, 2)[:, 1] for e in edge_lists])
+    rel_e = torch.cat([torch.full((int(e.reshape(-1, 2).shape[0]),), r, dtype=torch.int16, device=dev)
+                       for r, e in enumerate(edge_lists)])
+    _, cols, rows, eid, indptr = ops.csr_build(dst, src, num_nodes)
+    return {"indptr": indptr, "cols": cols, "rows": rows, "eid": eid, "rel": rel_e.index_select(0, eid),
+            "src": src, "dst": dst, "rel_e": rel_e}
+
+
 def typed_csr(edge_lists, num_nodes):
     """The relation-typed CSRs of edge lists ``edge_lists[r]`` ([E_r, 2] int64 CUDA tensors, (src, dst) rows) over
-    ``num_nodes`` nodes.  The relations' edges are concatenated in order and run through the stable ``ops.csr_build``,
-    so the slots of every row come out grouped by relation in ascending relation id, ascending eid inside a group.
+    ``num_nodes`` nodes, on ``typed_in_csr``'s layout.
 
     fwd (dst-keyed): indptr, cols (src), rel (int16 relation per slot); the run list of the weight gradient --
     run_row / run_beg / run_end of every (row, relation) group, sorted by relation (stable), run_off [R + 1] --
@@ -248,13 +263,10 @@ def typed_csr(edge_lists, num_nodes):
     bwd (src-keyed): indptr, cols (dst), rel, w = 1 / cnt_r(dst) per slot."""
     R = len(edge_lists)
     dev = edge_lists[0].device
-    src = torch.cat([e.reshape(-1, 2)[:, 0] for e in edge_lists])
-    dst = torch.cat([e.reshape(-1, 2)[:, 1] for e in edge_lists])
-    rel_e = torch.cat([torch.full((int(e.reshape(-1, 2).shape[0]),), r, dtype=torch.int16, device=dev)
-                       for r, e in enumerate(edge_lists)])
+    t = typed_in_csr(edge_lists, num_nodes)
+    src, dst, rel_e = t["src"], t["dst"], t["rel_e"]
+    cols, rows, eid, indptr, rel = t["cols"], t["rows"], t["eid"], t["indptr"], t["rel"]
     E = int(src.shape[0])
-    _, cols, rows, eid, indptr = ops.csr_build(dst, src, num_nodes)
-    rel = rel_e.index_select(0, eid)
     brk = torch.ones(E, dtype=torch.bool, device=dev)
     if E > 1:
         brk[1:] = (rel[1:] != rel[:-1]) | (rows[1:] != rows[:-1])

@@ -1950,6 +1950,10 @@ def _aligned16(t):
 def _rgcn_agg_raw(csr, x2, w3, slot_w=None):
     """pglb_rgcn_agg_f32: out[d] = sum_r A_r[d] w3[r] on a typed CSR (heter_graph.typed_csr)."""
     n, K, N = csr["n_rows"], int(w3.shape[1]), int(w3.shape[2])
+    if int(csr["cols"].shape[0]) == 0:
+        # no edges (a sampled block whose targets have no in-edges): every run is empty, so every row is 0 -- what the
+        # kernel would write; its empty slot arrays have no address to pass
+        return torch.zeros((n, N), dtype=torch.float32, device=x2.device)
     out = torch.empty((n, N), dtype=torch.float32, device=x2.device)
     with torch.cuda.device(x2.device):
         check(lib.pglb_rgcn_agg_f32(_ptr(csr["indptr"]), _ptr(csr["cols"]), _ptr(csr["rel"]), _ptr(slot_w), _ptr(x2),
