@@ -672,6 +672,26 @@ int pglb_node2vec_walk(const int64_t *indptr, const int64_t *cols, const int64_t
 int pglb_walk_host(const int64_t *indptr, const int64_t *cols, const int64_t *sorted_cols, int64_t num_nodes,
                    const int64_t *nodes, int64_t n, int64_t max_depth, double p, double q, int mode, uint64_t seed,
                    int64_t *out, uint64_t *stats);
+/* Metapath walks on a heterogeneous graph (replace the reference's examples/metapath2vec/datasets/sampling.py
+ * metapath_randomwalk).  indptrs / cols are host arrays of m pointers, 1 <= m <= 64: position k of the metapath is a
+ * relation's src-keyed CSR (indptrs[k], cols[k]) over the same num_nodes nodes; a relation may fill several positions.
+ * Pass indptrs[k] in place of a relation's empty cols (it is never read).
+ *   - Walker i starts at nodes[i] and writes row i of out (row-major, L = walk_length columns): at most walk_length
+ *     nodes, then -1.  Step t (t = 0, 1, ...) goes from cur to the uniform slot of cur's row in relation position
+ *     t % m, drawn as a random_walk step: mulhi64(r64, deg) with r64 from Philox4x32-10(counter = (i lo32, i hi32, t,
+ *     0), key = (seed lo32, seed hi32)).  So m = 1 gives pglb_random_walk's walks bit for bit.
+ *   - A walk ends early exactly when cur has no out-edge in the step's relation.  A start outside [0, num_nodes) gives
+ *     a row of -1.  Nothing checks that the relations chain by node type.
+ *   - m outside [1, 64], walk_length outside [1, 2^31 - 1), a negative size, or a NULL pointer with n > 0 (indptrs,
+ *     cols, any of their first m entries, nodes, out): PGLB_EINVAL before any CUDA call.
+ * pglb_metapath_walk: device pointers in indptrs / cols, nodes and out; one launch on `stream`.
+ * pglb_metapath_walk_host: the same walks over host arrays by the kernel's own walk function, one walker after
+ * another, blocking.  For tests and small graphs. */
+int pglb_metapath_walk(const int64_t *const *indptrs, const int64_t *const *cols, int m, int64_t num_nodes,
+                       const int64_t *nodes, int64_t n, int64_t walk_length, uint64_t seed, int64_t *out,
+                       void *stream);
+int pglb_metapath_walk_host(const int64_t *const *indptrs, const int64_t *const *cols, int m, int64_t num_nodes,
+                            const int64_t *nodes, int64_t n, int64_t walk_length, uint64_t seed, int64_t *out);
 
 /* ------------------------------------------------------------------------------------
  * Graph-level readouts (csrc/readout.cu).  Every entry is keyed by a segment CSR indptr[B + 1] (device int64,

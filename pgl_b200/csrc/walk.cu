@@ -17,6 +17,10 @@
 //     same draw as a random_walk step.
 // walk_step is the only statement of one step; the kernels and pglb_walk_host all call walk_one, which calls it.
 //
+// Metapath walks (pglb_metapath_walk; the reference's examples/metapath2vec metapath_randomwalk): step t follows
+// relation metapath[t % m], each relation its own src-keyed CSR, and is walk_uniform's step on that relation's row
+// with the draw of (walker, t, trial 0).  With m = 1 a metapath walk is therefore a random_walk bit for bit.
+//
 // Membership ("near") is a binary search in the row-sorted copy of the successor columns (`sorted`: same indptr, each
 // row ascending by id).  node2vec: one search in prev's row per trial, O(log deg(prev)).  node2vec_plus: one search in
 // the row of every earlier node, O(t log d) per trial at step t -- the walk's own output row is its history.
@@ -116,10 +120,10 @@ __host__ __device__ __forceinline__ int walk_class(const int64_t *indptr, const 
 }
 
 // the uniform slot of trial 0: a random_walk step, and the first step of a node2vec walk
-__host__ __device__ __forceinline__ int64_t walk_uniform(const WalkRule &r, const int64_t *cols, uint32_t t,
+__host__ __device__ __forceinline__ int64_t walk_uniform(uint64_t seed, const int64_t *cols, uint32_t t,
                                                          uint64_t walker, int64_t b, int64_t deg, WalkStats &st) {
     st.trials += 1;
-    return walk_ld(cols + b + (int64_t)walk_mulhi64(walk_r64(walk_draw(r.seed, walker, t, 0)), (uint64_t)deg));
+    return walk_ld(cols + b + (int64_t)walk_mulhi64(walk_r64(walk_draw(seed, walker, t, 0)), (uint64_t)deg));
 }
 
 // Step t of walker `walker` from the row [b, b + deg) (deg > 0) of cur = hist[t], prev = hist[t - 1]: the next node.
@@ -128,8 +132,8 @@ __host__ __device__ __forceinline__ int64_t walk_step(const WalkRule &r, const i
                                                       const int64_t *sorted, const int64_t *hist, uint32_t t,
                                                       uint64_t walker, int64_t b, int64_t deg, int64_t prev,
                                                       WalkStats &st) {
-    if constexpr (MODE == WALK_UNIFORM) return walk_uniform(r, cols, t, walker, b, deg, st);
-    if (t == 0) return walk_uniform(r, cols, t, walker, b, deg, st);
+    if constexpr (MODE == WALK_UNIFORM) return walk_uniform(r.seed, cols, t, walker, b, deg, st);
+    if (t == 0) return walk_uniform(r.seed, cols, t, walker, b, deg, st);
     const int64_t cap = deg > WALK_TRIALS ? deg : WALK_TRIALS;
     for (int64_t k = 0; k < cap; ++k) {
         const uint4 d = walk_draw(r.seed, walker, t, (uint32_t)k);
@@ -226,6 +230,76 @@ int walk_launch(const char *name, const int64_t *indptr, const int64_t *cols, co
     return PGLB_OK;
 }
 
+// A metapath's relations travel into the kernel by value, as one __grid_constant__ parameter of about 1 KB: a step
+// reads its (indptr, cols) pair from the parameter bank with a dynamic index (a constant-memory load, no local copy),
+// so it costs what a random_walk step costs.
+constexpr int METAPATH_MAX = 64;
+
+struct MetapathRule {
+    uint64_t seed;
+    int m;  // 1 <= m <= METAPATH_MAX
+    const int64_t *indptr[METAPATH_MAX];
+    const int64_t *cols[METAPATH_MAX];
+};
+
+// The whole metapath walk of one walker into out[0, L): start, then up to L - 1 steps, then -1 padding.  A start
+// outside [0, num_nodes) gives a row of -1, as in walk_one.
+__host__ __device__ __forceinline__ void metapath_one(const MetapathRule &r, int64_t num_nodes, int64_t start,
+                                                      uint64_t walker, int64_t *out, int64_t L) {
+    WalkStats st{0, 0};  // walk_uniform counts its draws; nothing reads the count here
+    int64_t k = 0;
+    if (start >= 0 && start < num_nodes) {
+        int64_t cur = start;
+        out[k++] = cur;
+        int pos = 0;  // t % m, kept as a wrapping counter instead of a division
+        for (int64_t t = 0; t + 1 < L; ++t) {
+            const int64_t *indptr = r.indptr[pos];
+            const int64_t b = walk_ld(indptr + cur);
+            const int64_t deg = walk_ld(indptr + cur + 1) - b;
+            if (deg == 0) break;
+            cur = walk_uniform(r.seed, r.cols[pos], (uint32_t)t, walker, b, deg, st);
+            out[k++] = cur;
+            if (++pos == r.m) pos = 0;
+        }
+    }
+    for (; k < L; ++k) out[k] = -1;
+}
+
+__global__ void __launch_bounds__(256) metapath_walk_kernel(const __grid_constant__ MetapathRule r, int64_t num_nodes,
+                                                            const int64_t *__restrict__ nodes, int64_t n,
+                                                            int64_t *__restrict__ out, int64_t L) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n)
+        metapath_one(r, num_nodes, __ldg(reinterpret_cast<const long long *>(nodes + i)), (uint64_t)i, out + i * L, L);
+}
+
+// the checks of both metapath entries, before anything else; walk_check's on every relation
+inline int metapath_check(const char *name, const int64_t *const *indptrs, const int64_t *const *cols, int m,
+                          int64_t num_nodes, const int64_t *nodes, int64_t n, int64_t walk_length, const int64_t *out) {
+    PGLB_CHECK_ARG(m >= 1 && m <= METAPATH_MAX, PGLB_EINVAL, "%s: m must lie in [1, %d], got %d", name, METAPATH_MAX,
+                   m);
+    PGLB_CHECK_ARG(walk_length >= 1 && walk_length < INT32_MAX, PGLB_EINVAL,
+                   "%s: walk_length must lie in [1, 2^31 - 1)", name);
+    PGLB_CHECK_ARG(n <= 0 || (indptrs && cols), PGLB_EINVAL, "%s: NULL pointer", name);
+    for (int k = 0; k < m; ++k)
+        if (const int rc = walk_check(name, n > 0 ? indptrs[k] : nullptr, n > 0 ? cols[k] : nullptr, nullptr,
+                                      num_nodes, nodes, n, walk_length, out, false, 1, 1))
+            return rc;
+    return PGLB_OK;
+}
+
+inline MetapathRule metapath_rule_of(const int64_t *const *indptrs, const int64_t *const *cols, int m,
+                                     uint64_t seed) {
+    MetapathRule r{};
+    r.seed = seed;
+    r.m = m;
+    for (int k = 0; k < m; ++k) {
+        r.indptr[k] = indptrs[k];
+        r.cols[k] = cols[k];
+    }
+    return r;
+}
+
 }  // namespace pglb
 
 using namespace pglb;
@@ -285,5 +359,32 @@ extern "C" int pglb_walk_host(const int64_t *indptr, const int64_t *cols, const 
         stats[0] = st.trials;
         stats[1] = st.fallbacks;
     }
+    return PGLB_OK;
+}
+
+extern "C" int pglb_metapath_walk(const int64_t *const *indptrs, const int64_t *const *cols, int m, int64_t num_nodes,
+                                  const int64_t *nodes, int64_t n, int64_t walk_length, uint64_t seed, int64_t *out,
+                                  void *stream) {
+    const char *name = "pglb_metapath_walk";
+    if (const int rc = metapath_check(name, indptrs, cols, m, num_nodes, nodes, n, walk_length, out)) return rc;
+    if (n == 0) return PGLB_OK;
+    const MetapathRule r = metapath_rule_of(indptrs, cols, m, seed);
+    const unsigned grid = (unsigned)((n + 255) / 256);
+    metapath_walk_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(r, num_nodes, nodes, n, out,
+                                                                                    walk_length);
+    PGLB_LAUNCH_CHECK("metapath_walk_kernel");
+    return PGLB_OK;
+}
+
+// The same walks on the host, one walker after another, through the kernel's metapath_one (include/pglb.h).
+extern "C" int pglb_metapath_walk_host(const int64_t *const *indptrs, const int64_t *const *cols, int m,
+                                       int64_t num_nodes, const int64_t *nodes, int64_t n, int64_t walk_length,
+                                       uint64_t seed, int64_t *out) {
+    const char *name = "pglb_metapath_walk_host";
+    if (const int rc = metapath_check(name, indptrs, cols, m, num_nodes, nodes, n, walk_length, out)) return rc;
+    if (n == 0) return PGLB_OK;
+    const MetapathRule r = metapath_rule_of(indptrs, cols, m, seed);
+    for (int64_t i = 0; i < n; ++i)
+        metapath_one(r, num_nodes, nodes[i], (uint64_t)i, out + i * walk_length, walk_length);
     return PGLB_OK;
 }

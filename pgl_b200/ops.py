@@ -200,6 +200,23 @@ def node2vec_walk(indptr, cols, sorted_cols, num_nodes, nodes, max_depth, p, q, 
     return out
 
 
+def metapath_walk(indptrs, cols_list, num_nodes, nodes, walk_length, seed):
+    """pglb_metapath_walk: [len(nodes), walk_length] int64 walks, -1 after a walk ends.  Step t follows the src-keyed
+    CSR (indptrs[t % m], cols_list[t % m]); the m CSRs share num_nodes and one device."""
+    nodes, _ = _walk_args(indptrs[0], cols_list[0], nodes)
+    cols_p = [_walk_args(ip, c, nodes)[1].value for ip, c in zip(indptrs, cols_list)]
+    if any(t.device != nodes.device for t in list(indptrs) + list(cols_list)):
+        raise ValueError("metapath_walk: the CSRs and the start nodes must be on one device")
+    m = len(cols_p)
+    indptr_arr = (ctypes.c_void_p * m)(*[ip.data_ptr() for ip in indptrs])
+    cols_arr = (ctypes.c_void_p * m)(*cols_p)
+    out = torch.empty((nodes.numel(), int(walk_length)), dtype=torch.int64, device=nodes.device)
+    with torch.cuda.device(nodes.device):
+        check(lib.pglb_metapath_walk(indptr_arr, cols_arr, m, int(num_nodes), _ptr(nodes), nodes.numel(),
+                                     int(walk_length), int(seed), _ptr(out), _stream()))
+    return out
+
+
 # graph-level readouts (csrc/readout.cu)
 # ------------------------------------------------------------------------------------------
 
