@@ -464,6 +464,70 @@ int pglb_dot_attn_bwd_edge_drop_x16(const int64_t *rows, const int64_t *cols, co
                                     float attn_drop, uint64_t seed, uint64_t offset, float *beta_e, float *ds_e,
                                     void *stream);
 
+/* Dot-product attention of TransformerConv WITH edge features (pgl/nn/conv.py:808-847 with edge_feat: the score of
+ * q[dst] * (k[src] + e) summed over the head dim, the weighted sum of v[src] + e) in ONE pass, as pglb_dot_attn_csr_*:
+ *   s_j = <q[d,h,:], k[cols[j],h,:] + e[eid[j],h,:]>,  lse[d,h] = log sum_j exp(s_j),
+ *   out[d,h,:] = sum_j exp(s_j - lse) (v[cols[j],h,:] + e[eid[j],h,:])
+ * (rows without in-edges: out = 0).  The add comes first, then the dot, both in float32, so e = 0 gives the
+ * pglb_dot_attn_csr_* output and lse bit for bit.
+ *   - The pglb_dot_attn_csr_* arguments, rules and return codes, plus eid [num_edges] (dst-CSR slot -> edge id, as the
+ *     edge backward's eid), e [num_edges, H * head_dim] in EDGE-ID order in q's dtype, row stride lde in elements.
+ *     NULL eid or e with edges: PGLB_EINVAL.  e not 16-byte aligned, lde below D or not a multiple of 16 bytes:
+ *     PGLB_ESHAPE.
+ *   - _x16 and _drop_: as pglb_dot_attn_csr_x16 / pglb_dot_attn_drop_csr_*; out == round16(the f32 entry on the
+ *     widened q, k, v, e), and with dropout out = sum_j s m_j exp(s_j - lse) (v_j + e_j), lse the value without it.
+ *   - All argument checks precede any CUDA call. */
+int pglb_dot_attn_e_csr_f32(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const float *q, int64_t ldq,
+                            const float *k, int64_t ldk, const float *v, int64_t ldv, const float *e, int64_t lde,
+                            float *out, int64_t ldo, float *lse, int64_t n_dst, int64_t n_src, int64_t num_edges,
+                            int64_t H, int64_t head_dim, void *ws, size_t ws_bytes, void *stream);
+int pglb_dot_attn_e_csr_x16(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const void *q, int64_t ldq,
+                            const void *k, int64_t ldk, const void *v, int64_t ldv, const void *e, int64_t lde,
+                            void *out, int64_t ldo, float *lse, int64_t n_dst, int64_t n_src, int64_t num_edges,
+                            int64_t H, int64_t head_dim, int dtype, void *ws, size_t ws_bytes, void *stream);
+int pglb_dot_attn_e_drop_csr_f32(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const float *q,
+                                 int64_t ldq, const float *k, int64_t ldk, const float *v, int64_t ldv, const float *e,
+                                 int64_t lde, float *out, int64_t ldo, float *lse, int64_t n_dst, int64_t n_src,
+                                 int64_t num_edges, int64_t H, int64_t head_dim, float attn_drop, uint64_t seed,
+                                 uint64_t offset, void *ws, size_t ws_bytes, void *stream);
+int pglb_dot_attn_e_drop_csr_x16(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const void *q,
+                                 int64_t ldq, const void *k, int64_t ldk, const void *v, int64_t ldv, const void *e,
+                                 int64_t lde, void *out, int64_t ldo, float *lse, int64_t n_dst, int64_t n_src,
+                                 int64_t num_edges, int64_t H, int64_t head_dim, int dtype, float attn_drop,
+                                 uint64_t seed, uint64_t offset, void *ws, size_t ws_bytes, void *stream);
+
+/* Per-edge part of that attention's backward: pglb_dot_attn_bwd_edge_* with k + e and v + e in place of k and v (s
+ * rebuilt bit for bit from the forward's score), plus the edge-feature gradient
+ *   grad_e[e,h,:] = ds_e[e,h] * q[dst,h,:] + beta_e[e,h] * G[dst,h,:]
+ * in e's dtype, each edge's row written once, no atomics.  e [num_edges, H * head_dim] in edge-id order (row stride
+ * lde); grad_e is nullable (e needs no gradient), row stride ldge.  The caller finishes grad q with one more
+ * aggregation, send_ue_recv(e, ds_e, mul, sum) over the dst-keyed CSR with eid as its column array; grad k and grad v
+ * are those of pglb_dot_attn_bwd_edge_*.  NULL e with edges: PGLB_EINVAL; e or grad_e not 16-byte aligned, lde or
+ * ldge below D or not a multiple of 16 bytes: PGLB_ESHAPE.  _x16 / _drop_ as there; grad_e == round16(the f32
+ * entry's on the widened inputs). */
+int pglb_dot_attn_e_bwd_edge_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *q,
+                                 int64_t ldq, const float *k, int64_t ldk, const float *v, int64_t ldv, const float *e,
+                                 int64_t lde, const float *grad_out, int64_t ldg, const float *out, int64_t ldo,
+                                 const float *lse, int64_t num_edges, int64_t H, int64_t head_dim, float *beta_e,
+                                 float *ds_e, float *grad_e, int64_t ldge, void *stream);
+int pglb_dot_attn_e_bwd_edge_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *q,
+                                 int64_t ldq, const void *k, int64_t ldk, const void *v, int64_t ldv, const void *e,
+                                 int64_t lde, const void *grad_out, int64_t ldg, const void *out, int64_t ldo,
+                                 const float *lse, int64_t num_edges, int64_t H, int64_t head_dim, int dtype,
+                                 float *beta_e, float *ds_e, void *grad_e, int64_t ldge, void *stream);
+int pglb_dot_attn_e_bwd_edge_drop_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *q,
+                                      int64_t ldq, const float *k, int64_t ldk, const float *v, int64_t ldv,
+                                      const float *e, int64_t lde, const float *grad_out, int64_t ldg, const float *out,
+                                      int64_t ldo, const float *lse, int64_t num_edges, int64_t H, int64_t head_dim,
+                                      float attn_drop, uint64_t seed, uint64_t offset, float *beta_e, float *ds_e,
+                                      float *grad_e, int64_t ldge, void *stream);
+int pglb_dot_attn_e_bwd_edge_drop_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *q,
+                                      int64_t ldq, const void *k, int64_t ldk, const void *v, int64_t ldv,
+                                      const void *e, int64_t lde, const void *grad_out, int64_t ldg, const void *out,
+                                      int64_t ldo, const float *lse, int64_t num_edges, int64_t H, int64_t head_dim,
+                                      int dtype, float attn_drop, uint64_t seed, uint64_t offset, float *beta_e,
+                                      float *ds_e, void *grad_e, int64_t ldge, void *stream);
+
 /* GATv2 attention (pgl/nn/conv.py:420-427: send_uv(feature, feature, add), LeakyReLU, the sum with attn over the head
  * dim, edge_softmax, attention dropout, send_ue_recv(mul, sum)) in ONE pass, the GAT kernel's online softmax:
  *   z_j = f[cols[j],h,:] + f[d,h,:],  s_j = sum_c a[h,c] lrelu(z_j,c),  lrelu(x) = max(x, slope x),

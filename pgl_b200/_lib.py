@@ -138,6 +138,25 @@ _SIGS = {
                                                 _i64, _i64, ctypes.c_float, _u64, _u64, _p, _p, _p]),
     "pglb_dot_attn_bwd_edge_drop_x16": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64,
                                                 _i64, _i64, c_int, ctypes.c_float, _u64, _u64, _p, _p, _p]),
+    "pglb_dot_attn_e_csr_f32": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _i64,
+                                        _i64, _i64, _i64, _p, c_size_t, _p]),
+    "pglb_dot_attn_e_csr_x16": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _i64,
+                                        _i64, _i64, _i64, c_int, _p, c_size_t, _p]),
+    "pglb_dot_attn_e_drop_csr_f32": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64,
+                                             _i64, _i64, _i64, _i64, ctypes.c_float, _u64, _u64, _p, c_size_t, _p]),
+    "pglb_dot_attn_e_drop_csr_x16": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64,
+                                             _i64, _i64, _i64, _i64, c_int, ctypes.c_float, _u64, _u64, _p, c_size_t,
+                                             _p]),
+    "pglb_dot_attn_e_bwd_edge_f32": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64,
+                                             _p, _i64, _i64, _i64, _p, _p, _p, _i64, _p]),
+    "pglb_dot_attn_e_bwd_edge_x16": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64,
+                                             _p, _i64, _i64, _i64, c_int, _p, _p, _p, _i64, _p]),
+    "pglb_dot_attn_e_bwd_edge_drop_f32": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p,
+                                                  _i64, _p, _i64, _i64, _i64, ctypes.c_float, _u64, _u64, _p, _p, _p,
+                                                  _i64, _p]),
+    "pglb_dot_attn_e_bwd_edge_drop_x16": (c_int, [_p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p, _i64, _p,
+                                                  _i64, _p, _i64, _i64, _i64, c_int, ctypes.c_float, _u64, _u64, _p,
+                                                  _p, _p, _i64, _p]),
     "pglb_gatv2_attn_csr_f32": (c_int, [_p, _p, _p, _i64, _p, ctypes.c_float, _p, _i64, _p, _i64, _i64, _i64, _i64,
                                         _p, c_size_t, _p]),
     "pglb_gatv2_attn_csr_x16": (c_int, [_p, _p, _p, _i64, _p, ctypes.c_float, _p, _i64, _p, _i64, _i64, _i64, _i64,

@@ -210,12 +210,18 @@ __global__ void __launch_bounds__(256) gat_bwd_edge_kernel(
 // in flight per lane.  s is formed by the forward's dot4_lane + head_sum_lanes, so it is the forward's score bit for bit.
 // T: element type of q, k, v, G and out (16-bit rows are widened exactly; everything after is the fp32 kernel's).
 // DROP: da = s m da and beta = m ? fl(a s) : 0 (m the slot and head's keep bit, s = 1 / (1 - p)); delta is unchanged.
-template <int LPH, typename T, bool DROP>
+// EF (pglb_dot_attn_e_*, launched as <LPH, T, DROP, true>): edge features e [E, D] in edge-id order; k + e and v + e
+// (add4, as the forward forms them) take the places of k and v, and grad_e (nullable) gets
+// grad_e[e,h,:] = ds q[dst,h,:] + beta G[dst,h,:], each edge's row written once by the lanes of its slot, in T.  EF is a
+// trailing pack so the instantiations without edge features keep their names, <LPH, T, DROP>, in profiles and traces.
+template <int LPH, typename T, bool DROP, bool... EF>
 __global__ void __launch_bounds__(256) dot_attn_bwd_edge_kernel(
     const int64_t *__restrict__ rows, const int64_t *__restrict__ cols, const int64_t *__restrict__ eid,
     const T *__restrict__ q, int64_t ldq, const T *__restrict__ k, int64_t ldk, const T *__restrict__ v, int64_t ldv,
     const T *__restrict__ g, int64_t ldg, const T *__restrict__ out, int64_t ldo, const float *__restrict__ lse,
-    int64_t E, int H, int D, float *__restrict__ beta_e, float *__restrict__ ds_e, const AttnDrop drop) {
+    int64_t E, int H, int D, float *__restrict__ beta_e, float *__restrict__ ds_e, const AttnDrop drop,
+    const T *__restrict__ e = nullptr, int64_t lde = 0, T *__restrict__ grad_e = nullptr, int64_t ldge = 0) {
+    constexpr bool kEF = (false || ... || EF);
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -249,6 +255,11 @@ __global__ void __launch_bounds__(256) dot_attn_bwd_edge_kernel(
                 if (k0 + u < cnt && act) {
                     kv[u] = ldg_row4<T>(k + cc * ldk + lane * 4);
                     vv[u] = ldg_row4<T>(v + cc * ldv + lane * 4);
+                    if constexpr (kEF) {
+                        const float4 e4 = ldg_row4<T>(e + ii[u] * lde + lane * 4);
+                        kv[u] = add4(kv[u], e4);
+                        vv[u] = add4(vv[u], e4);
+                    }
                 }
             }
 #pragma unroll
@@ -277,6 +288,17 @@ __global__ void __launch_bounds__(256) dot_attn_bwd_edge_kernel(
                 if (lead) {
                     beta_e[ii[u] * H + head] = beta;
                     ds_e[ii[u] * H + head] = a * (da - delta);
+                }
+                if constexpr (kEF) {
+                    if (grad_e && act) {
+                        const float ds = a * (da - delta);
+                        const float4 ge = make_float4(fmaf(beta, g4.x, ds * q4.x), fmaf(beta, g4.y, ds * q4.y),
+                                                      fmaf(beta, g4.z, ds * q4.z), fmaf(beta, g4.w, ds * q4.w));
+                        if constexpr (sizeof(T) == 4)
+                            __stcs(reinterpret_cast<float4 *>(grad_e + ii[u] * ldge + lane * 4), ge);
+                        else
+                            __stcs(reinterpret_cast<uint2 *>(grad_e + ii[u] * ldge + lane * 4), round4<T>(ge));
+                    }
                 }
             }
         }
@@ -564,17 +586,21 @@ extern "C" int pglb_gat_bwd_edge_drop_x16(const int64_t *rows, const int64_t *co
 }
 
 // The checks and the launch of the dot-product attention's edge-backward entries (include/pglb.h).  T: element type of
-// q, k, v, grad_out and out, rows 16-byte aligned.  drop (nullable): the attention-dropout stream (H % 4 == 0 then).
+// q, k, v, e, grad_out, out and grad_e, rows 16-byte aligned.  drop (nullable): the attention-dropout stream (H % 4 == 0
+// then).  ef: an edge-feature entry (pglb_dot_attn_e_bwd_edge_*, the kernel's EF): e must be given, grad_e is
+// nullable.
 template <typename T>
 static int dot_attn_bwd_edge_entry(const char *name, const int64_t *rows, const int64_t *cols, const int64_t *eid,
                                    const void *q_, int64_t ldq, const void *k_, int64_t ldk, const void *v_, int64_t ldv,
                                    const void *g_, int64_t ldg, const void *out_, int64_t ldo, const float *lse,
                                    int64_t num_edges, int64_t H, int64_t head_dim, float *beta_e, float *ds_e,
-                                   void *stream_, const AttnDrop *drop) {
+                                   void *stream_, const AttnDrop *drop, bool ef = false, const void *e_ = nullptr,
+                                   int64_t lde = 0, void *grad_e_ = nullptr, int64_t ldge = 0) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     const T *q = reinterpret_cast<const T *>(q_), *k = reinterpret_cast<const T *>(k_),
             *v = reinterpret_cast<const T *>(v_), *g = reinterpret_cast<const T *>(g_),
-            *out = reinterpret_cast<const T *>(out_);
+            *out = reinterpret_cast<const T *>(out_), *e = reinterpret_cast<const T *>(e_);
+    T *grad_e = reinterpret_cast<T *>(grad_e_);
     constexpr int64_t B = sizeof(T);
     PGLB_CHECK_ARG(num_edges >= 0 && H > 0 && head_dim > 0, PGLB_EINVAL, "%s: bad size", name);
     const int64_t D = H * head_dim;
@@ -583,18 +609,29 @@ static int dot_attn_bwd_edge_entry(const char *name, const int64_t *rows, const 
                    "%s: needs H*head_dim <= 128 and head_dim in {4, 8, 16, 32, 64, 128}", name);
     PGLB_CHECK_ARG(!drop || H % 4 == 0, PGLB_EUNSUPPORTED, "%s: needs H %% 4 == 0", name);
     if (num_edges == 0) return PGLB_OK;
-    PGLB_CHECK_ARG(rows && cols && q && k && v && g && out && lse && beta_e && ds_e, PGLB_EINVAL, "%s: NULL pointer",
-                   name);
+    PGLB_CHECK_ARG(rows && cols && q && k && v && g && out && lse && beta_e && ds_e && (!ef || e), PGLB_EINVAL,
+                   "%s: NULL pointer", name);
     auto a16 = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
     PGLB_CHECK_ARG(ldq >= D && ldk >= D && ldv >= D && ldg >= D && ldo >= D && (ldq * B) % 16 == 0 &&
                        (ldk * B) % 16 == 0 && (ldv * B) % 16 == 0 && (ldg * B) % 16 == 0 && (ldo * B) % 16 == 0 &&
                        a16(q) && a16(k) && a16(v) && a16(g) && a16(out),
                    PGLB_ESHAPE, "%s: rows must be 16-byte aligned", name);
+    PGLB_CHECK_ARG(!ef || (lde >= D && (lde * B) % 16 == 0 && a16(e) &&
+                           (!grad_e || (ldge >= D && (ldge * B) % 16 == 0 && a16(grad_e)))),
+                   PGLB_ESHAPE, "%s: e / grad_e rows must be 16-byte aligned", name);
     const int grid = grid_of(num_edges, 64);  // a warp per 32 slots, grid-stride
     const AttnDrop dr = drop ? *drop : AttnDrop{};
 #define PGLB_DBE(L)                                                                                                   \
     do {                                                                                                              \
-        if (drop)                                                                                                     \
+        if (ef && drop)                                                                                               \
+            dot_attn_bwd_edge_kernel<L, T, true, true><<<grid, 256, 0, stream>>>(                                     \
+                rows, cols, eid, q, ldq, k, ldk, v, ldv, g, ldg, out, ldo, lse, num_edges, (int)H, (int)D, beta_e,    \
+                ds_e, dr, e, lde, grad_e, ldge);                                                                      \
+        else if (ef)                                                                                                  \
+            dot_attn_bwd_edge_kernel<L, T, false, true><<<grid, 256, 0, stream>>>(                                    \
+                rows, cols, eid, q, ldq, k, ldk, v, ldv, g, ldg, out, ldo, lse, num_edges, (int)H, (int)D, beta_e,    \
+                ds_e, dr, e, lde, grad_e, ldge);                                                                      \
+        else if (drop)                                                                                                \
             dot_attn_bwd_edge_kernel<L, T, true><<<grid, 256, 0, stream>>>(rows, cols, eid, q, ldq, k, ldk, v, ldv,   \
                                                                            g, ldg, out, ldo, lse, num_edges, (int)H,  \
                                                                            (int)D, beta_e, ds_e, dr);                 \
@@ -670,6 +707,74 @@ extern "C" int pglb_dot_attn_bwd_edge_drop_x16(const int64_t *rows, const int64_
                                                       ldo, lse, num_edges, H, head_dim, beta_e, ds_e, stream_, &drop);
     return dot_attn_bwd_edge_entry<__half>(name, rows, cols, eid, q, ldq, k, ldk, v, ldv, grad_out, ldg, out, ldo, lse,
                                            num_edges, H, head_dim, beta_e, ds_e, stream_, &drop);
+}
+
+// Edge backward with edge features (include/pglb.h): the pglb_dot_attn_bwd_edge_* arguments plus e [num_edges, H *
+// head_dim] in edge-id order (row stride lde) and grad_e (nullable, row stride ldge).
+extern "C" int pglb_dot_attn_e_bwd_edge_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid,
+                                            const float *q, int64_t ldq, const float *k, int64_t ldk, const float *v,
+                                            int64_t ldv, const float *e, int64_t lde, const float *grad_out,
+                                            int64_t ldg, const float *out, int64_t ldo, const float *lse,
+                                            int64_t num_edges, int64_t H, int64_t head_dim, float *beta_e, float *ds_e,
+                                            float *grad_e, int64_t ldge, void *stream_) {
+    return dot_attn_bwd_edge_entry<float>("pglb_dot_attn_e_bwd_edge_f32", rows, cols, eid, q, ldq, k, ldk, v, ldv,
+                                          grad_out, ldg, out, ldo, lse, num_edges, H, head_dim, beta_e, ds_e, stream_,
+                                          nullptr, true, e, lde, grad_e, ldge);
+}
+
+extern "C" int pglb_dot_attn_e_bwd_edge_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid,
+                                            const void *q, int64_t ldq, const void *k, int64_t ldk, const void *v,
+                                            int64_t ldv, const void *e, int64_t lde, const void *grad_out,
+                                            int64_t ldg, const void *out, int64_t ldo, const float *lse,
+                                            int64_t num_edges, int64_t H, int64_t head_dim, int dtype, float *beta_e,
+                                            float *ds_e, void *grad_e, int64_t ldge, void *stream_) {
+    const char *name = "pglb_dot_attn_e_bwd_edge_x16";
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    if (dtype == PGLB_DTYPE_BF16)
+        return dot_attn_bwd_edge_entry<__nv_bfloat16>(name, rows, cols, eid, q, ldq, k, ldk, v, ldv, grad_out, ldg, out,
+                                                      ldo, lse, num_edges, H, head_dim, beta_e, ds_e, stream_, nullptr,
+                                                      true, e, lde, grad_e, ldge);
+    return dot_attn_bwd_edge_entry<__half>(name, rows, cols, eid, q, ldq, k, ldk, v, ldv, grad_out, ldg, out, ldo, lse,
+                                           num_edges, H, head_dim, beta_e, ds_e, stream_, nullptr, true, e, lde,
+                                           grad_e, ldge);
+}
+
+extern "C" int pglb_dot_attn_e_bwd_edge_drop_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid,
+                                                 const float *q, int64_t ldq, const float *k, int64_t ldk,
+                                                 const float *v, int64_t ldv, const float *e, int64_t lde,
+                                                 const float *grad_out, int64_t ldg, const float *out, int64_t ldo,
+                                                 const float *lse, int64_t num_edges, int64_t H, int64_t head_dim,
+                                                 float attn_drop, uint64_t seed, uint64_t offset, float *beta_e,
+                                                 float *ds_e, float *grad_e, int64_t ldge, void *stream_) {
+    const char *name = "pglb_dot_attn_e_bwd_edge_drop_f32";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    return dot_attn_bwd_edge_entry<float>(name, rows, cols, eid, q, ldq, k, ldk, v, ldv, grad_out, ldg, out, ldo, lse,
+                                          num_edges, H, head_dim, beta_e, ds_e, stream_, &drop, true, e, lde, grad_e,
+                                          ldge);
+}
+
+extern "C" int pglb_dot_attn_e_bwd_edge_drop_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid,
+                                                 const void *q, int64_t ldq, const void *k, int64_t ldk,
+                                                 const void *v, int64_t ldv, const void *e, int64_t lde,
+                                                 const void *grad_out, int64_t ldg, const void *out, int64_t ldo,
+                                                 const float *lse, int64_t num_edges, int64_t H, int64_t head_dim,
+                                                 int dtype, float attn_drop, uint64_t seed, uint64_t offset,
+                                                 float *beta_e, float *ds_e, void *grad_e, int64_t ldge,
+                                                 void *stream_) {
+    const char *name = "pglb_dot_attn_e_bwd_edge_drop_x16";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    if (dtype == PGLB_DTYPE_BF16)
+        return dot_attn_bwd_edge_entry<__nv_bfloat16>(name, rows, cols, eid, q, ldq, k, ldk, v, ldv, grad_out, ldg, out,
+                                                      ldo, lse, num_edges, H, head_dim, beta_e, ds_e, stream_, &drop,
+                                                      true, e, lde, grad_e, ldge);
+    return dot_attn_bwd_edge_entry<__half>(name, rows, cols, eid, q, ldq, k, ldk, v, ldv, grad_out, ldg, out, ldo, lse,
+                                           num_edges, H, head_dim, beta_e, ds_e, stream_, &drop, true, e, lde, grad_e,
+                                           ldge);
 }
 
 // The checks and the launch of the GATv2 edge-backward entries (include/pglb.h).  T: element type of f, grad_out and

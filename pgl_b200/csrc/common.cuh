@@ -147,6 +147,11 @@ __device__ __forceinline__ float4 ldg_row4(const T *p) {
 __device__ __forceinline__ float dot4_lane(const float4 &a, const float4 &b) {
     return fmaf(a.w, b.w, fmaf(a.z, b.z, fmaf(a.y, b.y, a.x * b.x)));
 }
+// the edge-feature operand of the dot-product attention (spmm_gat5_kernel<kScoreDotE>, dot_attn_bwd_edge_kernel<EF>):
+// k + e and v + e, formed the same way in the forward and the backward
+__device__ __forceinline__ float4 add4(const float4 &a, const float4 &b) {
+    return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+}
 __device__ __forceinline__ float head_sum_lanes(float v, int lph) {
 #pragma unroll
     for (int o = 16; o >= 1; o >>= 1)

@@ -484,14 +484,16 @@ int gat_fused_run(const int64_t *indptr, const int64_t *cols, const void *f, int
                   size_t ws_bytes, cudaStream_t stream);
 template <typename T>
 bool gat5_takes(int64_t D, float slope, const void *f, int64_t ldf, const float *attn_src, int64_t H, int64_t n_src);
-// the fused dot-product attention (TransformerConv) over q / k / v / out of element type T, and whether it takes a call
+// the fused dot-product attention (TransformerConv) over q / k / v / out of element type T, with edge features e
+// (nullable, through eid), and whether it takes a call
 template <typename T>
 int dot_attn_run(const int64_t *indptr, const int64_t *cols, const void *q, int64_t ldq, const void *k, int64_t ldk,
-                 const void *v, int64_t ldv, void *out, int64_t ldo, float *lse, int64_t n_dst, int64_t E, int64_t H,
-                 int64_t head_dim, const AttnDrop *drop, void *ws, size_t ws_bytes, cudaStream_t stream);
+                 const void *v, int64_t ldv, const int64_t *eid, const void *e, int64_t lde, void *out, int64_t ldo,
+                 float *lse, int64_t n_dst, int64_t E, int64_t H, int64_t head_dim, const AttnDrop *drop, void *ws,
+                 size_t ws_bytes, cudaStream_t stream);
 template <typename T>
 bool dot_attn_takes(int64_t D, int64_t head_dim, const void *q, int64_t ldq, const void *k, int64_t ldk, const void *v,
-                    int64_t ldv, int64_t n_src);
+                    int64_t ldv, const void *e, int64_t lde, int64_t n_src);
 
 // the fused GATv2 attention (GATv2Conv) over f / out of element type T, and whether it takes a call
 template <typename T>
@@ -1114,12 +1116,14 @@ extern "C" int pglb_gat_fused_train_drop_csr_x16(const int64_t *indptr, const in
 }
 
 // The argument checks and the launch of the dot-product attention entries (include/pglb.h).  T: element type of q, k,
-// v and out.  Every check precedes any CUDA call.  drop (nullable): the attention-dropout stream.
+// v, e and out.  Every check precedes any CUDA call.  drop (nullable): the attention-dropout stream.  ef: an edge-feature
+// entry (pglb_dot_attn_e_*), whose eid and e must then be given when there are edges.
 template <typename T>
 static int dot_attn_entry(const char *name, const int64_t *indptr, const int64_t *cols, const void *q, int64_t ldq,
                           const void *k, int64_t ldk, const void *v, int64_t ldv, void *out, int64_t ldo, float *lse,
                           int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H, int64_t head_dim, void *ws,
-                          size_t ws_bytes, void *stream_, const AttnDrop *drop) {
+                          size_t ws_bytes, void *stream_, const AttnDrop *drop, bool ef = false,
+                          const int64_t *eid = nullptr, const void *e = nullptr, int64_t lde = 0) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     constexpr int64_t B = sizeof(T);
     PGLB_CHECK_ARG(n_dst >= 0 && n_src >= 0 && num_edges >= 0 && H > 0 && head_dim > 0, PGLB_EINVAL, "%s: bad size", name);
@@ -1132,17 +1136,17 @@ static int dot_attn_entry(const char *name, const int64_t *indptr, const int64_t
     if (n_dst == 0) return PGLB_OK;
     PGLB_CHECK_ARG(indptr && out, PGLB_EINVAL, "%s: NULL pointer", name);
     PGLB_CHECK_ARG(ldq >= D && ldk >= D && ldv >= D && ldo >= D && (ldo * B) % 16 == 0 && aligned16(out) &&
-                       dot_attn_takes<T>(D, head_dim, q, ldq, k, ldk, v, ldv, n_src),
+                       (!ef || lde >= D) && dot_attn_takes<T>(D, head_dim, q, ldq, k, ldk, v, ldv, e, lde, n_src),
                    PGLB_ESHAPE, "%s: rows must be 16-byte aligned", name);
     if (num_edges == 0) {
         PGLB_CUDA(cudaMemset2DAsync(out, B * ldo, 0, B * D, n_dst, stream));
         return PGLB_OK;
     }
-    PGLB_CHECK_ARG(cols && q && k && v, PGLB_EINVAL, "%s: NULL pointer", name);
+    PGLB_CHECK_ARG(cols && q && k && v && (!ef || (eid && e)), PGLB_EINVAL, "%s: NULL pointer", name);
     PGLB_CHECK_ARG(ws && (reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
                    "%s: workspace NULL or not 256-byte aligned", name);
-    return dot_attn_run<T>(indptr, cols, q, ldq, k, ldk, v, ldv, out, ldo, lse, n_dst, num_edges, H, head_dim, drop, ws,
-                           ws_bytes, stream);
+    return dot_attn_run<T>(indptr, cols, q, ldq, k, ldk, v, ldv, eid, e, lde, out, ldo, lse, n_dst, num_edges, H,
+                           head_dim, drop, ws, ws_bytes, stream);
 }
 
 extern "C" int pglb_dot_attn_csr_f32(const int64_t *indptr, const int64_t *cols, const float *q, int64_t ldq,
@@ -1194,6 +1198,65 @@ extern "C" int pglb_dot_attn_drop_csr_x16(const int64_t *indptr, const int64_t *
         using T = std::remove_pointer_t<decltype(elem)>;
         return dot_attn_entry<T>(name, indptr, cols, q, ldq, k, ldk, v, ldv, out, ldo, lse, n_dst, n_src, num_edges, H,
                                  head_dim, ws, ws_bytes, stream_, &drop);
+    };
+    return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
+}
+
+// Dot-product attention with edge features (include/pglb.h): the pglb_dot_attn_* arguments plus eid (dst-CSR slot ->
+// edge id), e [num_edges, H * head_dim] in edge-id order and its row stride lde.
+extern "C" int pglb_dot_attn_e_csr_f32(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const float *q,
+                                       int64_t ldq, const float *k, int64_t ldk, const float *v, int64_t ldv,
+                                       const float *e, int64_t lde, float *out, int64_t ldo, float *lse, int64_t n_dst,
+                                       int64_t n_src, int64_t num_edges, int64_t H, int64_t head_dim, void *ws,
+                                       size_t ws_bytes, void *stream_) {
+    return dot_attn_entry<float>("pglb_dot_attn_e_csr_f32", indptr, cols, q, ldq, k, ldk, v, ldv, out, ldo, lse, n_dst,
+                                 n_src, num_edges, H, head_dim, ws, ws_bytes, stream_, nullptr, true, eid, e, lde);
+}
+
+extern "C" int pglb_dot_attn_e_csr_x16(const int64_t *indptr, const int64_t *cols, const int64_t *eid, const void *q,
+                                       int64_t ldq, const void *k, int64_t ldk, const void *v, int64_t ldv,
+                                       const void *e, int64_t lde, void *out, int64_t ldo, float *lse, int64_t n_dst,
+                                       int64_t n_src, int64_t num_edges, int64_t H, int64_t head_dim, int dtype,
+                                       void *ws, size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_dot_attn_e_csr_x16";
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    auto run = [&](auto *elem) -> int {
+        using T = std::remove_pointer_t<decltype(elem)>;
+        return dot_attn_entry<T>(name, indptr, cols, q, ldq, k, ldk, v, ldv, out, ldo, lse, n_dst, n_src, num_edges, H,
+                                 head_dim, ws, ws_bytes, stream_, nullptr, true, eid, e, lde);
+    };
+    return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
+}
+
+extern "C" int pglb_dot_attn_e_drop_csr_f32(const int64_t *indptr, const int64_t *cols, const int64_t *eid,
+                                            const float *q, int64_t ldq, const float *k, int64_t ldk, const float *v,
+                                            int64_t ldv, const float *e, int64_t lde, float *out, int64_t ldo,
+                                            float *lse, int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H,
+                                            int64_t head_dim, float attn_drop, uint64_t seed, uint64_t offset,
+                                            void *ws, size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_dot_attn_e_drop_csr_f32";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    return dot_attn_entry<float>(name, indptr, cols, q, ldq, k, ldk, v, ldv, out, ldo, lse, n_dst, n_src, num_edges, H,
+                                 head_dim, ws, ws_bytes, stream_, &drop, true, eid, e, lde);
+}
+
+extern "C" int pglb_dot_attn_e_drop_csr_x16(const int64_t *indptr, const int64_t *cols, const int64_t *eid,
+                                            const void *q, int64_t ldq, const void *k, int64_t ldk, const void *v,
+                                            int64_t ldv, const void *e, int64_t lde, void *out, int64_t ldo,
+                                            float *lse, int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t H,
+                                            int64_t head_dim, int dtype, float attn_drop, uint64_t seed,
+                                            uint64_t offset, void *ws, size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_dot_attn_e_drop_csr_x16";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    auto run = [&](auto *elem) -> int {
+        using T = std::remove_pointer_t<decltype(elem)>;
+        return dot_attn_entry<T>(name, indptr, cols, q, ldq, k, ldk, v, ldv, out, ldo, lse, n_dst, n_src, num_edges, H,
+                                 head_dim, ws, ws_bytes, stream_, &drop, true, eid, e, lde);
     };
     return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
 }

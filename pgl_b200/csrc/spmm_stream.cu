@@ -1286,17 +1286,21 @@ int gat_fused_run(const int64_t *indptr, const int64_t *cols, const void *f, int
 
 template <typename T>
 bool dot_attn_takes(int64_t D, int64_t head_dim, const void *q, int64_t ldq, const void *k, int64_t ldk, const void *v,
-                    int64_t ldv, int64_t n_src) {
+                    int64_t ldv, const void *e, int64_t lde, int64_t n_src) {
+    if (e) return dot_attn_e_eligible<T>(D, head_dim, q, ldq, k, ldk, v, ldv, e, lde, n_src);
     return dot_attn_eligible<T>(D, head_dim, q, ldq, k, ldk, v, ldv, n_src);
 }
 
 // Single-pass dot-product attention (TransformerConv): out[d,h,:] = sum_j softmax_j(<q[d,h,:], k[src_j,h,:]>) v[src_j,h,:]
-// on spmm_gat5_kernel<DOT>.  T: element type of q, k, v and out; the call is one dot_attn_takes accepts.  lse
-// (nullable): the rows' log-sum-exp.  drop (nullable): the attention-dropout stream.
+// on spmm_gat5_kernel<DOT>.  With edge features e (nullable; [E, D] in edge-id order, eid the dst-CSR's slot -> edge
+// id): k + e and v + e in place of k and v, on spmm_gat5_kernel<DOTE>.  T: element type of q, k, v, e and out; the
+// call is one dot_attn_takes accepts.  lse (nullable): the rows' log-sum-exp.  drop (nullable): the attention-dropout
+// stream.
 template <typename T>
 int dot_attn_run(const int64_t *indptr, const int64_t *cols, const void *q, int64_t ldq, const void *k, int64_t ldk,
-                 const void *v, int64_t ldv, void *out, int64_t ldo, float *lse, int64_t n_dst, int64_t E, int64_t H,
-                 int64_t head_dim, const AttnDrop *drop, void *ws, size_t ws_bytes, cudaStream_t stream) {
+                 const void *v, int64_t ldv, const int64_t *eid, const void *e, int64_t lde, void *out, int64_t ldo,
+                 float *lse, int64_t n_dst, int64_t E, int64_t H, int64_t head_dim, const AttnDrop *drop, void *ws,
+                 size_t ws_bytes, cudaStream_t stream) {
     StreamP p{};
     p.ldy = H;
     p.head_dim = (int)head_dim;
@@ -1311,6 +1315,8 @@ int dot_attn_run(const int64_t *indptr, const int64_t *cols, const void *q, int6
         const int rc = launch_empty_rows<T>(p, stream);
         if (rc) return rc;
     }
+    if (e && drop) return launch_dot_attn_e<T, true>(p, q, ldq, k, ldk, eid, e, lde, *drop, stream);
+    if (e) return launch_dot_attn_e<T, false>(p, q, ldq, k, ldk, eid, e, lde, AttnDrop{}, stream);
     if (drop) return launch_dot_attn<T, true>(p, q, ldq, k, ldk, *drop, stream);
     return launch_dot_attn<T, false>(p, q, ldq, k, ldk, AttnDrop{}, stream);
 }

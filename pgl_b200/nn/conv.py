@@ -433,12 +433,12 @@ class GCNII(nn.Module):
 
 
 class TransformerConv(nn.Module):
-    """reference pgl/nn/conv.py:724-885.  Without edge features on a ``Graph`` the reference's UDF
-    pair (send q[dst]*k[src] summed over the head dim -> recv softmax, dropout, weight v, reduce) is
-    one fused pass with a fused backward (``ops.dot_attention``); shapes those kernels refuse are
-    lowered to ``send_uv(mul)`` -> sum -> ``edge_softmax`` -> ``send_ue_recv(mul, sum)`` (no second
-    gather of v by edge id, no zero+scatter); with edge features it runs the send/recv pair like
-    the reference."""
+    """reference pgl/nn/conv.py:724-885.  On a ``Graph`` the reference's UDF pair (send
+    q[dst]*(k[src] + e) summed over the head dim -> recv softmax, dropout, weight v[src] + e, reduce)
+    is one fused pass with a fused backward (``ops.dot_attention``), with or without edge features e.
+    Shapes those kernels refuse are lowered, without edge features, to ``send_uv(mul)`` -> sum ->
+    ``edge_softmax`` -> ``send_ue_recv(mul, sum)`` (no second gather of v by edge id, no
+    zero+scatter); with edge features they run the send/recv pair like the reference."""
 
     def __init__(self, input_size, hidden_size, num_heads=4, feat_drop=0.6, attn_drop=0.6,
                  concat=True, skip_feat=True, gate=False, layer_norm=True, activation="relu"):
@@ -482,17 +482,18 @@ class TransformerConv(nn.Module):
 
     def send_recv(self, graph, q, k, v, edge_feat):
         q = q / (self.hidden_size ** 0.5)
-        if edge_feat is not None:
-            msg = graph.send(self.send_attention, src_feat={"k": k, "v": v}, dst_feat={"q": q},
-                             edge_feat={"edge_feat": edge_feat})
-            return graph.recv(reduce_func=self.reduce_attention, msg=msg)
         output = None
         if type(graph).__name__ == "Graph" and q.is_cuda:
             # score, softmax, dropout and weighted sum in one pass with a fused backward (ops._DotAttn): no [E, H*Dh]
             # product; None when the shape is outside the kernels
             from .. import ops
             drop = self.attn_drop if self.attn_drop > 1e-15 and self.training else 0.0
-            output = ops.dot_attention(graph._fwd_csr(), graph._bwd_csr, q, k, v, attn_drop=drop)
+            output = ops.dot_attention(graph._fwd_csr(), graph._bwd_csr, q, k, v, attn_drop=drop,
+                                       edge_feat=edge_feat)
+        if output is None and edge_feat is not None:
+            msg = graph.send(self.send_attention, src_feat={"k": k, "v": v}, dst_feat={"q": q},
+                             edge_feat={"edge_feat": edge_feat})
+            return graph.recv(reduce_func=self.reduce_attention, msg=msg)
         if output is None:
             alpha = torch.sum(graph.send_uv(k, q, "mul"), dim=-1)
             alpha = GF.edge_softmax(graph, alpha).reshape(-1, self.num_heads, 1)

@@ -1723,8 +1723,9 @@ def gat_fused_train(fwd, bwd, f, attn_src, attn_dst, negative_slope=0.2, out_dty
     return out if out.dtype == res else out.to(res)
 
 
-def _dot_attn_fwd_raw(fwd, q2, k2, v2, H, Dh, drop, want_lse):
-    """pglb_dot_attn_* on [N, H*Dh] rows of one dtype: (out, lse or None)."""
+def _dot_attn_fwd_raw(fwd, q2, k2, v2, H, Dh, drop, want_lse, e2=None):
+    """pglb_dot_attn_* on [N, H*Dh] rows of one dtype: (out, lse or None).  e2: edge features [E, H*Dh] in edge-id
+    order (pglb_dot_attn_e_*)."""
     n = int(q2.shape[0])
     E = int(fwd["cols"].shape[0])
     out = torch.empty((n, H * Dh), dtype=q2.dtype, device=q2.device)
@@ -1732,11 +1733,17 @@ def _dot_attn_fwd_raw(fwd, q2, k2, v2, H, Dh, drop, want_lse):
     need = ctypes.c_size_t(0)
     check(lib.pglb_spmm_csr_ws(n, E, H * Dh, ctypes.byref(need)))
     ws = workspace(q2.device, need.value)
-    args = (_ptr(fwd["indptr"]), _ptr(fwd["cols"]), _ptr(q2), q2.stride(0), _ptr(k2), k2.stride(0), _ptr(v2),
-            v2.stride(0), _ptr(out), out.stride(0), _ptr(lse), n, n, E, H, Dh)
+    ef = () if e2 is None else (_ptr(fwd["eid"]),)
+    rows = (_ptr(q2), q2.stride(0), _ptr(k2), k2.stride(0), _ptr(v2), v2.stride(0))
+    if e2 is not None:
+        rows += (_ptr(e2), e2.stride(0))
+    args = (_ptr(fwd["indptr"]), _ptr(fwd["cols"]), *ef, *rows, _ptr(out), out.stride(0), _ptr(lse), n, n, E, H, Dh)
     dt = (_DTYPE16[q2.dtype],) if q2.dtype in HALF_DTYPES else ()
     fn = {(False, False): lib.pglb_dot_attn_csr_f32, (False, True): lib.pglb_dot_attn_csr_x16,
           (True, False): lib.pglb_dot_attn_drop_csr_f32, (True, True): lib.pglb_dot_attn_drop_csr_x16}
+    if e2 is not None:
+        fn = {(False, False): lib.pglb_dot_attn_e_csr_f32, (False, True): lib.pglb_dot_attn_e_csr_x16,
+              (True, False): lib.pglb_dot_attn_e_drop_csr_f32, (True, True): lib.pglb_dot_attn_e_drop_csr_x16}
     with torch.cuda.device(q2.device):
         check(fn[(drop is not None, bool(dt))](*args, *dt, *(drop or ()), _ptr(ws), ws.numel(), _stream()))
     return out, lse
@@ -1748,20 +1755,22 @@ class _DotAttn(torch.autograd.Function):
     lse[N, H]).  Backward = one edge kernel (pglb_dot_attn_bwd_edge_*: scores and weights rebuilt, two head dots per
     edge) + three aggregations on the existing send_ue_recv kernels.  16-bit rows take the *_x16 entries; lse, beta and
     ds are float32 and the gradients are in the rows' dtype.  drop = (p, seed, offset): attention dropout recomputed from
-    (seed, offset) in the forward and the backward."""
+    (seed, offset) in the forward and the backward.  e2 (None or edge features [E, H*Dh] in edge-id order): the
+    pglb_dot_attn_e_* entries, k + e and v + e in place of k and v; the edge kernel also writes grad e, and grad q
+    takes one more aggregation, of e by edge id."""
 
     @staticmethod
-    def forward(ctx, q2, k2, v2, fwd, bwd, H, Dh, drop):
-        out, lse = _dot_attn_fwd_raw(fwd, q2, k2, v2, H, Dh, drop, True)
+    def forward(ctx, q2, k2, v2, e2, fwd, bwd, H, Dh, drop):
+        out, lse = _dot_attn_fwd_raw(fwd, q2, k2, v2, H, Dh, drop, True, e2)
         ctx.meta = (fwd, bwd, H, Dh, drop)
-        ctx.save_for_backward(q2, k2, v2, out, lse)
+        ctx.save_for_backward(q2, k2, v2, e2, out, lse)
         return out
 
     @staticmethod
     def backward(ctx, g):
         fwd, bwd, H, Dh, drop = ctx.meta
         bwd = bwd() if callable(bwd) else bwd
-        q2, k2, v2, out, lse = ctx.saved_tensors
+        q2, k2, v2, e2, out, lse = ctx.saved_tensors
         half = q2.dtype in HALF_DTYPES
         g = _f32_2d(g.to(q2.dtype) if g.dtype != q2.dtype else g, allow16=half)
         E = int(fwd["cols"].shape[0])
@@ -1769,33 +1778,47 @@ class _DotAttn(torch.autograd.Function):
         beta = torch.empty((E, H), dtype=torch.float32, device=g.device)
         ds = torch.empty((E, H), dtype=torch.float32, device=g.device)
         dt = (_DTYPE16[q2.dtype],) if half else ()
-        fn = {(False, False): lib.pglb_dot_attn_bwd_edge_f32, (False, True): lib.pglb_dot_attn_bwd_edge_x16,
-              (True, False): lib.pglb_dot_attn_bwd_edge_drop_f32, (True, True): lib.pglb_dot_attn_bwd_edge_drop_x16}
+        rows = (_ptr(q2), q2.stride(0), _ptr(k2), k2.stride(0), _ptr(v2), v2.stride(0))
+        ge, ef = None, ()
+        if e2 is None:
+            fn = {(False, False): lib.pglb_dot_attn_bwd_edge_f32, (False, True): lib.pglb_dot_attn_bwd_edge_x16,
+                  (True, False): lib.pglb_dot_attn_bwd_edge_drop_f32, (True, True): lib.pglb_dot_attn_bwd_edge_drop_x16}
+        else:
+            fn = {(False, False): lib.pglb_dot_attn_e_bwd_edge_f32, (False, True): lib.pglb_dot_attn_e_bwd_edge_x16,
+                  (True, False): lib.pglb_dot_attn_e_bwd_edge_drop_f32,
+                  (True, True): lib.pglb_dot_attn_e_bwd_edge_drop_x16}
+            rows += (_ptr(e2), e2.stride(0))
+            ge = torch.empty_like(e2) if ctx.needs_input_grad[3] else None
+            ef = (_ptr(ge), H * Dh)
         with torch.cuda.device(g.device):
             check(fn[(drop is not None, half)](
-                _ptr(fwd["rows"]), _ptr(fwd["cols"]), _ptr(fwd["eid"]), _ptr(q2), q2.stride(0), _ptr(k2), k2.stride(0),
-                _ptr(v2), v2.stride(0), _ptr(g), g.stride(0), _ptr(out), out.stride(0), _ptr(lse), E, H, Dh, *dt,
-                *(drop or ()), _ptr(beta), _ptr(ds), _stream()))
+                _ptr(fwd["rows"]), _ptr(fwd["cols"]), _ptr(fwd["eid"]), *rows, _ptr(g), g.stride(0), _ptr(out),
+                out.stride(0), _ptr(lse), E, H, Dh, *dt, *(drop or ()), _ptr(beta), _ptr(ds), *ef, _stream()))
         gq = gk = gv = None
 
         def agg(csr, x2, w):   # sum over the CSR's slots of w[eid, head] * x2[col]
             return _spmm_raw(csr["indptr"], csr["cols"], x2, n, "sum", eid=csr["eid"], y2=w, y_bcast=BCAST_HEAD,
                              head_dim=Dh, msg_op="mul", max_degree=csr.get("max_degree", -1))
-        if ctx.needs_input_grad[0]:   # grad q[d] = sum over the in-edges of d of ds k[src]
+        if ctx.needs_input_grad[0]:   # grad q[d] = sum over the in-edges of d of ds k[src] (+ ds e[eid])
             gq = agg(fwd, k2, ds)
+            if e2 is not None:        # the e rows are addressed by edge id: the CSR's eid is their column array
+                gq += agg({"indptr": fwd["indptr"], "cols": fwd["eid"], "eid": fwd["eid"],
+                           "max_degree": fwd.get("max_degree", -1)}, e2, ds)
         if ctx.needs_input_grad[1]:   # grad k[u] = sum over the out-edges of u of ds q[dst]
             gk = agg(bwd, q2, ds)
         if ctx.needs_input_grad[2]:   # grad v[u] = sum over the out-edges of u of beta G[dst]
             gv = agg(bwd, g, beta)
-        return gq, gk, gv, None, None, None, None, None
+        return gq, gk, gv, ge, None, None, None, None, None
 
 
-def dot_attention(fwd, bwd, q, k, v, attn_drop=0.0, seed=None):
-    """TransformerConv's attention without edge features in one pass:
+def dot_attention(fwd, bwd, q, k, v, attn_drop=0.0, seed=None, edge_feat=None):
+    """TransformerConv's attention in one pass:
     out[d,h,:] = sum over the in-edges j of d of softmax_j(<q[d,h,:], k[src_j,h,:]>) v[src_j,h,:]
-    (q already scaled by 1 / sqrt(Dh)), with a fused backward when autograd needs one.  q, k, v [N, H, Dh] of one dtype
-    (float32, bfloat16 or float16) on one graph (n_dst == N); ``fwd`` is the dst-keyed CSR dict (with ``rows``),
-    ``bwd`` the src-keyed one or a callable returning it.  Returns [N, H, Dh] in that dtype, or None when the call is
+    (q already scaled by 1 / sqrt(Dh)), with a fused backward when autograd needs one.  ``edge_feat`` [E, H, Dh] in
+    edge-id order, q's dtype: k + e and v + e in place of k[src_j] and v[src_j] (the add first, then the dot), and the
+    backward also returns grad edge_feat; None when it has another shape or dtype, or rows that are not 16-byte
+    aligned.  q, k, v [N, H, Dh] of one dtype (float32, bfloat16 or float16) on one graph (n_dst == N); ``fwd`` is
+    the dst-keyed CSR dict (with ``rows``), ``bwd`` the src-keyed one or a callable returning it.  Returns [N, H, Dh] in that dtype, or None when the call is
     outside the kernels (H*Dh > 128, Dh not a power of two >= 4, rows the kernels cannot read, mixed dtypes, float64, no
     edges, attn_drop >= 1, dropout during CUDA-graph capture); the caller then keeps the op-by-op path.
     ``attn_drop`` in (0, 1): dropout on the normalised attention per edge and head inside the kernels, the mask drawn
@@ -1817,16 +1840,24 @@ def dot_attention(fwd, bwd, q, k, v, attn_drop=0.0, seed=None):
         return None     # the generator's offset advances on the host: not replayable by a graph
     if int(fwd["indptr"].shape[0]) - 1 != n or int(fwd["cols"].shape[0]) == 0 or fwd.get("rows") is None:
         return None
+    e2 = None
+    if edge_feat is not None:
+        require_cuda(edge_feat)
+        if edge_feat.dtype != q.dtype or tuple(edge_feat.shape) != (int(fwd["cols"].shape[0]), H, Dh):
+            return None
+        e2 = _f32_2d(edge_feat, allow16=True)
+        if e2.data_ptr() % 16:
+            return None
     q2, k2, v2 = (_f32_2d(t, allow16=True) for t in (q, k, v))
     if any(t.data_ptr() % 16 for t in (q2, k2, v2)):
         return None
     drop = None
     if attn_drop > 0.0:
         drop = (attn_drop,) + (tuple(int(s) for s in seed) if seed is not None else _attn_drop_stream(q2.device))
-    if torch.is_grad_enabled() and any(t.requires_grad for t in (q, k, v)):
-        out = _DotAttn.apply(q2, k2, v2, fwd, bwd, H, Dh, drop)
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (q, k, v, edge_feat)):
+        out = _DotAttn.apply(q2, k2, v2, e2, fwd, bwd, H, Dh, drop)
     else:
-        out = _dot_attn_fwd_raw(fwd, q2, k2, v2, H, Dh, drop, False)[0]
+        out = _dot_attn_fwd_raw(fwd, q2, k2, v2, H, Dh, drop, False, e2)[0]
     return out.reshape(n, H, Dh)
 
 

@@ -1,0 +1,391 @@
+"""TransformerConv's fused dot-product attention with edge features (pglb_dot_attn_e_*, ops.dot_attention(edge_feat=)).
+
+Contract: for dst row d, head h and the in-edges j of d (edge id eid_j, source src_j),
+s_j = <q[d,h,:], k[src_j,h,:] + e[eid_j,h,:]> (q already scaled), lse = log sum_j exp(s_j),
+out[d,h,:] = sum_j exp(s_j - lse) (v[src_j,h,:] + e[eid_j,h,:]) (rows without in-edges: 0).  With dropout (keep bits m
+of the GAT stream, keyed by dst-CSR slot and head; s = 1 / (1 - p)) out = sum_j s m_j a_j (v_j + e_j) and lse is the
+value without dropout.  e is [E, H, Dh] in edge-id order.  The references are torch restatements of that contract:
+float64 for the float32 kernels, the float32 kernel on widened inputs for the 16-bit ones (bit for bit), plain torch
+fp32 with the library's mask for dropout; and, with e = 0, the entries without edge features, bit for bit."""
+import pytest
+import torch
+
+from oracle import oracle as O
+from test_gpu_exact_routes import _kernels_of
+from test_gpu_transformer_attn import (DTYPES, EMPTY, GRAD_TOL, LAYOUTS, SEED, U, _bits, _ends, _qkv, _rand, _s32,
+                                       bwd_raw, edge_mask, fwd_raw, graph, pgl, rel_err)  # noqa: F401 (fixtures)
+
+pytestmark = pytest.mark.gpu
+
+
+def _e(E, H, Dh, seed, dtype=torch.float32):
+    return _rand((E, H, Dh), seed, dtype, 0.5)
+
+
+def restate_e(q, k, v, e, src, dst, n, mask=None, s=1.0):
+    """The contract in torch, differentiable, in q's dtype: (out, lse); lse is -inf on empty rows."""
+    sc = (q[dst] * (k[src] + e)).sum(-1)
+    H = sc.shape[1]
+    m = torch.full((n, H), -float("inf"), dtype=sc.dtype, device=sc.device)
+    m = m.scatter_reduce(0, dst[:, None].expand(-1, H), sc, "amax")
+    pe = torch.exp(sc - m[dst])
+    l_ = torch.zeros((n, H), dtype=sc.dtype, device=sc.device).index_add(0, dst, pe)
+    a = pe / l_[dst]
+    beta = a if mask is None else a * mask * torch.tensor(s, dtype=sc.dtype, device=sc.device)
+    out = torch.zeros_like(v).index_add(0, dst, (v[src] + e) * beta.unsqueeze(-1))
+    return out, m + torch.log(l_)
+
+
+def fwd_raw_e(pgl, csr, q, k, v, e, drop=None):
+    n, H, Dh = q.shape
+    return pgl.ops._dot_attn_fwd_raw(csr, q.reshape(n, -1), k.reshape(n, -1), v.reshape(n, -1), H, Dh, drop, True,
+                                     e.reshape(e.shape[0], -1))
+
+
+def bwd_raw_e(pgl, csr, q, k, v, e, go, out, lse, drop=None):
+    """The edge-feature edge backward entry of q's dtype: (beta_e, ds_e, grad_e) in edge order."""
+    ops = pgl.ops
+    n, H, Dh = q.shape
+    q2, k2, v2, g2, o2 = (t.reshape(n, -1) for t in (q, k, v, go, out))
+    e2 = e.reshape(e.shape[0], -1)
+    E = int(csr["cols"].shape[0])
+    beta = torch.empty((E, H), device="cuda")
+    ds = torch.empty((E, H), device="cuda")
+    ge = torch.empty_like(e2)
+    dt = () if q.dtype == torch.float32 else (ops._DTYPE16[q.dtype],)
+    name = "pglb_dot_attn_e_bwd_edge_%s%s" % ("drop_" if drop else "", "x16" if dt else "f32")
+    ops.check(getattr(ops.lib, name)(
+        ops._ptr(csr["rows"]), ops._ptr(csr["cols"]), ops._ptr(csr["eid"]), ops._ptr(q2), q2.stride(0), ops._ptr(k2),
+        k2.stride(0), ops._ptr(v2), v2.stride(0), ops._ptr(e2), e2.stride(0), ops._ptr(g2), g2.stride(0),
+        ops._ptr(o2), o2.stride(0), ops._ptr(lse), E, H, Dh, *dt, *(drop or ()), ops._ptr(beta), ops._ptr(ds),
+        ops._ptr(ge), ge.stride(0), ops._stream()))
+    return beta, ds, ge
+
+
+def test_fixture_edge_ids_are_not_slots(pgl, graph):
+    g, _ = graph
+    eid = g._fwd_csr()["eid"]
+    assert not torch.equal(eid.cpu(), torch.arange(eid.numel()))
+
+
+@pytest.mark.parametrize("dyn", ["0", "2"])   # PGLB_GAT_DYN: static task map and the device-side queue
+@pytest.mark.parametrize("H,Dh", LAYOUTS)
+def test_forward_and_lse_against_float64(pgl, graph, monkeypatch, dyn, H, Dh):
+    monkeypatch.setenv("PGLB_GAT_DYN", dyn)
+    g, edges = graph
+    N, E = g.num_nodes, len(edges)
+    src, dst = _ends(edges)
+    q, k, v = _qkv(N, H, Dh, 13 * H + Dh)
+    e = _e(E, H, Dh, 17 * H + Dh)
+    out, lse = fwd_raw_e(pgl, g._fwd_csr(), q, k, v, e)
+    want, wlse = restate_e(q.double(), k.double(), v.double(), e.double(), src, dst, N)
+    got = out.reshape(N, H, Dh)
+    assert (got[-EMPTY:] == 0).all()
+    assert float((got.double() - want).abs().max()) <= 1e-4 * float(want.abs().max())
+    has = torch.isfinite(wlse)
+    assert float((lse.double()[has] - wlse[has]).abs().max()) <= 1e-4 * max(1.0, float(wlse[has].abs().max()))
+    assert (lse[~has] == 0).all()    # rows without in-edges are not written
+    inf = pgl.ops.dot_attention(g._fwd_csr(), g._bwd_csr, q, k, v, edge_feat=e)
+    assert torch.equal(_bits(inf), _bits(got))
+
+
+@pytest.mark.parametrize("drop", [None, (0.3,) + SEED])
+@pytest.mark.parametrize("dtype", (torch.float32,) + DTYPES)
+@pytest.mark.parametrize("H,Dh", [(8, 16), (4, 32), (32, 4)])
+def test_zero_edge_features_match_the_entries_without(pgl, graph, dtype, drop, H, Dh):
+    """k + 0 and v + 0 are exact and the add comes before the dot: e = 0 gives the pglb_dot_attn_* results bit for
+    bit, forward (out, lse) and edge backward (beta, ds)."""
+    g, edges = graph
+    N, E = g.num_nodes, len(edges)
+    fwd = g._fwd_csr()
+    q, k, v = _qkv(N, H, Dh, 19 * H + Dh, dtype)
+    z = torch.zeros((E, H, Dh), device="cuda", dtype=dtype)
+    out_e, lse_e = fwd_raw_e(pgl, fwd, q, k, v, z, drop)
+    out0, lse0 = fwd_raw(pgl, fwd, q, k, v, drop)
+    assert torch.equal(_bits(out_e), _bits(out0)) and torch.equal(_bits(lse_e), _bits(lse0))
+    go = _rand((N, H, Dh), 21, dtype)
+    o = out0.reshape(N, H, Dh)
+    b_e, d_e, ge = bwd_raw_e(pgl, fwd, q, k, v, z, go, o, lse0, drop)
+    b0, d0 = bwd_raw(pgl, fwd, q, k, v, go, o, lse0, drop)
+    assert torch.equal(_bits(b_e), _bits(b0)) and torch.equal(_bits(d_e), _bits(d0))
+    assert torch.isfinite(ge.float()).all()
+
+
+@pytest.mark.parametrize("H,Dh", LAYOUTS)
+def test_gradients_against_float64_autograd(pgl, graph, H, Dh):
+    g, edges = graph
+    N, E = g.num_nodes, len(edges)
+    src, dst = _ends(edges)
+    q, k, v = (t.requires_grad_() for t in _qkv(N, H, Dh, 29 * H + Dh))
+    e = _e(E, H, Dh, 31 * H + Dh).requires_grad_()
+    go = _rand((N, H, Dh), 5)
+    out = pgl.ops.dot_attention(g._fwd_csr(), g._bwd_csr, q, k, v, edge_feat=e)
+    got = torch.autograd.grad(out, (q, k, v, e), go, retain_graph=True)
+    again = torch.autograd.grad(out, (q, k, v, e), go)
+    q64, k64, v64, e64 = (t.detach().double().requires_grad_() for t in (q, k, v, e))
+    want = torch.autograd.grad(restate_e(q64, k64, v64, e64, src, dst, N)[0], (q64, k64, v64, e64), go.double())
+    for name, a, a2, b in zip("qkve", got, again, want):
+        assert a.dtype == torch.float32 and rel_err(a, b) <= GRAD_TOL, (name, rel_err(a, b))
+        assert torch.equal(_bits(a), _bits(a2)), name    # no atomics: the same bits on every pass
+    # only e needs a gradient: grad_e alone, the same bits
+    ge_only = torch.autograd.grad(pgl.ops.dot_attention(g._fwd_csr(), g._bwd_csr, q.detach(), k.detach(), v.detach(),
+                                                        edge_feat=e), e, go)[0]
+    assert torch.equal(_bits(ge_only), _bits(got[3]))
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("H,Dh", [(8, 16), (4, 32), (2, 64), (8, 8), (16, 4), (32, 4)])
+def test_x16_bit_exact_against_fp32_kernel(pgl, graph, dtype, H, Dh):
+    g, edges = graph
+    N, E = g.num_nodes, len(edges)
+    fwd = g._fwd_csr()
+    q, k, v = _qkv(N, H, Dh, 37 * H + Dh, dtype)
+    e = _e(E, H, Dh, 39 * H + Dh, dtype)
+    out16, lse16 = fwd_raw_e(pgl, fwd, q, k, v, e)
+    out32, lse32 = fwd_raw_e(pgl, fwd, q.float(), k.float(), v.float(), e.float())
+    assert out16.dtype == dtype
+    assert torch.equal(_bits(out16), _bits(out32.to(dtype)))
+    assert torch.equal(_bits(lse16), _bits(lse32))
+    go = _rand((N, H, Dh), 7, dtype)
+    o = out16.reshape(N, H, Dh)
+    b16, d16, g16 = bwd_raw_e(pgl, fwd, q, k, v, e, go, o, lse16)
+    b32, d32, g32 = bwd_raw_e(pgl, fwd, q.float(), k.float(), v.float(), e.float(), go.float(), o.float(), lse16)
+    assert torch.equal(_bits(b16), _bits(b32)) and torch.equal(_bits(d16), _bits(d32))
+    assert g16.dtype == dtype and torch.equal(_bits(g16), _bits(g32.to(dtype)))
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("H,Dh", [(8, 16), (4, 32), (16, 4)])
+def test_x16_gradients_against_fp32_autograd(pgl, graph, dtype, H, Dh):
+    """Within 4 u of the largest |grad| of fp32 torch autograd on the widened inputs, as without edge features."""
+    g, edges = graph
+    N, E = g.num_nodes, len(edges)
+    src, dst = _ends(edges)
+    q, k, v = (t.requires_grad_() for t in _qkv(N, H, Dh, 43 * H + Dh, dtype))
+    e = _e(E, H, Dh, 47 * H + Dh, dtype).requires_grad_()
+    go = _rand((N, H, Dh), 9, dtype)
+    out = pgl.ops.dot_attention(g._fwd_csr(), g._bwd_csr, q, k, v, edge_feat=e)
+    assert out.dtype == dtype
+    got = torch.autograd.grad(out, (q, k, v, e), go)
+    q32, k32, v32, e32 = (t.detach().float().requires_grad_() for t in (q, k, v, e))
+    want = torch.autograd.grad(restate_e(q32, k32, v32, e32, src, dst, N)[0], (q32, k32, v32, e32), go.float())
+    for name, a, b in zip("qkve", got, want):
+        assert a.dtype == dtype and rel_err(a, b) <= 4 * U[dtype], (name, rel_err(a, b))
+
+
+@pytest.mark.parametrize("H,Dh", [(8, 16), (4, 8), (32, 4)])
+def test_dropout(pgl, graph, H, Dh):
+    g, edges = graph
+    N, E = g.num_nodes, len(edges)
+    fwd = g._fwd_csr()
+    src, dst = _ends(edges)
+    p = 0.3
+    drop = (p,) + SEED
+    mask, s = edge_mask(fwd, H, p), _s32(p)
+    q, k, v = _qkv(N, H, Dh, 53 * H + Dh)
+    e = _e(E, H, Dh, 59 * H + Dh)
+    out, lse = fwd_raw_e(pgl, fwd, q, k, v, e, drop)
+    _, lse0 = fwd_raw_e(pgl, fwd, q, k, v, e)
+    assert torch.equal(_bits(lse), _bits(lse0))              # lse is the value without dropout
+    want, _ = restate_e(q, k, v, e, src, dst, N, mask, s)
+    assert rel_err(out.reshape(N, H, Dh), want) <= 1e-4
+    # the backward recomputes the same mask from (seed, offset): gradients against torch fp32 with that mask
+    qg, kg, vg, eg = (t.clone().requires_grad_() for t in (q, k, v, e))
+    go = _rand((N, H, Dh), 13)
+    o = pgl.ops.dot_attention(fwd, g._bwd_csr, qg, kg, vg, attn_drop=p, seed=SEED, edge_feat=eg)
+    assert torch.equal(_bits(o.detach().reshape(N, -1)), _bits(out))
+    got = torch.autograd.grad(o, (qg, kg, vg, eg), go)
+    q2, k2, v2, e2 = (t.clone().requires_grad_() for t in (q, k, v, e))
+    want_g = torch.autograd.grad(restate_e(q2, k2, v2, e2, src, dst, N, mask, s)[0], (q2, k2, v2, e2), go)
+    for name, a, b in zip("qkve", got, want_g):
+        assert rel_err(a, b) <= GRAD_TOL, (name, rel_err(a, b))
+    for dtype in DTYPES:   # 16-bit dropout: the fp32 entries on the widened inputs, rounded
+        qh, kh, vh, eh = (t.to(dtype) for t in (q, k, v, e))
+        o16, l16 = fwd_raw_e(pgl, fwd, qh, kh, vh, eh, drop)
+        o32, l32 = fwd_raw_e(pgl, fwd, qh.float(), kh.float(), vh.float(), eh.float(), drop)
+        assert torch.equal(_bits(o16), _bits(o32.to(dtype))) and torch.equal(_bits(l16), _bits(l32))
+        goh = go.to(dtype)
+        r16 = bwd_raw_e(pgl, fwd, qh, kh, vh, eh, goh, o16.reshape(N, H, Dh), l16, drop)
+        r32 = bwd_raw_e(pgl, fwd, qh.float(), kh.float(), vh.float(), eh.float(), goh.float(),
+                        o16.reshape(N, H, Dh).float(), l16, drop)
+        assert all(torch.equal(_bits(a), _bits(b.to(a.dtype))) for a, b in zip(r16, r32))
+
+
+def test_calls_outside_the_kernels_return_none(pgl, graph):
+    g, edges = graph
+    N, E = g.num_nodes, len(edges)
+    fwd, bwd = g._fwd_csr(), g._bwd_csr
+    q, k, v = _qkv(N, 4, 8, 61)
+    e = _e(E, 4, 8, 62)
+    da = pgl.ops.dot_attention
+    assert da(fwd, bwd, q, k, v, edge_feat=e) is not None
+    assert da(fwd, bwd, q, k, v, edge_feat=e[:-1]) is None                     # not one row per edge
+    assert da(fwd, bwd, q, k, v, edge_feat=e[:, :1]) is None                   # broadcast over heads
+    assert da(fwd, bwd, q, k, v, edge_feat=e.reshape(E, 32)) is None           # [E, H*Dh]
+    assert da(fwd, bwd, q, k, v, edge_feat=e.half()) is None                   # dtype differs from q / k / v
+    assert da(fwd, bwd, q, k, v, edge_feat=e.double()) is None
+    assert da(fwd, bwd, q.double(), k.double(), v.double(), edge_feat=e.double()) is None
+    buf = torch.zeros(E * 32 + 1, device="cuda")
+    assert da(fwd, bwd, q, k, v, edge_feat=buf[1:].view(E, 4, 8)) is None      # rows not 16-byte aligned
+    assert da(fwd, bwd, *_qkv(N, 4, 12, 63), edge_feat=_e(E, 4, 12, 64)) is None   # head_dim not a power of two
+    assert da(fwd, bwd, *_qkv(N, 16, 16, 65), edge_feat=_e(E, 16, 16, 66)) is None  # 256 per row
+    assert da(fwd, bwd, *_qkv(N, 2, 16, 67), attn_drop=0.5, edge_feat=_e(E, 2, 16, 68)) is None   # H % 4
+    assert da(fwd, bwd, q, k, v, attn_drop=1.0, edge_feat=e) is None
+
+
+def _layer_ref(conv, g, edges, x, e):
+    """TransformerConv.forward (feat_drop = attn_drop = 0, skip, layer norm, relu) restated in float64 torch."""
+    H, Dh = conv.num_heads, conv.hidden_size
+    N = g.num_nodes
+    lin = {n: (m.weight.double(), m.bias.double()) for n, m in (("q", conv.q), ("k", conv.k), ("v", conv.v))}
+    x64 = x.double()
+    q, k, v = ((x64 @ lin[n][0] + lin[n][1]).reshape(N, H, Dh) for n in "qkv")   # weights are [in, out]
+    src, dst = _ends(edges)
+    out = restate_e(q / Dh ** 0.5, k, v, e.double().reshape(-1, H, Dh), src, dst, N)[0].reshape(N, -1)
+    out = out + x64 @ conv.skip_feat.weight.double() + conv.skip_feat.bias.double()
+    out = torch.nn.functional.layer_norm(out, (H * Dh,), conv.layer_norm.weight.double(),
+                                         conv.layer_norm.bias.double(), conv.layer_norm.eps)
+    return torch.relu(out)
+
+
+def test_declined_layer_still_matches_the_contract(pgl, graph):
+    """head_dim 12 is outside the kernels: the layer keeps the send / recv pair and still computes the contract."""
+    g, edges = graph
+    N, E = g.num_nodes, len(edges)
+    torch.manual_seed(5)
+    conv = pgl.nn.TransformerConv(32, 12, num_heads=4, feat_drop=0.0, attn_drop=0.0).cuda()
+    x = _rand((N, 32), 73)
+    e = _rand((E, 48), 74, scale=0.5)
+    calls = []
+    real = pgl.ops.dot_attention
+
+    def counted(*a, **kw):
+        r = real(*a, **kw)
+        calls.append(r is not None)
+        return r
+    pgl.ops.dot_attention = counted
+    try:
+        with torch.no_grad():
+            out = conv(g, x, e)
+    finally:
+        pgl.ops.dot_attention = real
+    assert calls == [False]
+    assert rel_err(out, _layer_ref(conv, g, edges, x, e)) <= 1e-4
+
+
+def _op_by_op(pgl, conv, g, *args):
+    """conv(g, *args) with ops.dot_attention declining every call: the layer's send / recv route."""
+    real = pgl.ops.dot_attention
+    pgl.ops.dot_attention = lambda *a, **kw: None
+    try:
+        return conv(g, *args)
+    finally:
+        pgl.ops.dot_attention = real
+
+
+@pytest.mark.parametrize("concat,gate", [(True, False), (True, True), (False, False), (False, True)])
+def test_layer_matches_the_op_by_op_route(pgl, graph, concat, gate):
+    g, edges = graph
+    N, E = g.num_nodes, len(edges)
+    torch.manual_seed(3)
+    H, Dh = 8, 16
+    conv = pgl.nn.TransformerConv(32, Dh, num_heads=H, feat_drop=0.0, attn_drop=0.0, concat=concat, gate=gate).cuda()
+    x = _rand((N, 32), 71)
+    e = _rand((E, H * Dh), 75, scale=0.5).requires_grad_()
+    go = _rand((N, H * Dh if concat else Dh), 72)
+    params = list(conv.parameters())
+    out = conv(g, x, e)
+    got = torch.autograd.grad(out, params + [e], go)
+    ref = _op_by_op(pgl, conv, g, x, e)
+    want = torch.autograd.grad(ref, params + [e], go)
+    assert rel_err(out, ref) <= 1e-4
+    scale = max(float(b.abs().max()) for b in want)
+    names = [n for n, _ in conv.named_parameters()] + ["edge_feat"]
+    for name, a, b in zip(names, got, want):
+        if name == "k.bias":   # shifts every score of a row alike: the exact gradient is 0, both routes give noise
+            assert float(a.abs().max()) <= 1e-4 * scale and float(b.abs().max()) <= 1e-4 * scale, name
+            continue
+        assert rel_err(a, b) <= 1e-4, (name, rel_err(a, b))
+
+
+def test_layer_reaches_the_edge_feature_entries_with_fewer_launches(pgl, graph, monkeypatch):
+    """Forward + backward of the layer: the fused route calls the edge-feature entries, once each and successfully,
+    and puts fewer launches on the device than the op-by-op route (whose gathers, adds and products are torch kernels,
+    not library launches).  The entries are observed at the C boundary, not through the profiler's kernel names."""
+    g, edges = graph
+    N, E = g.num_nodes, len(edges)
+    ops = pgl.ops
+    conv = pgl.nn.TransformerConv(32, 16, num_heads=8, feat_drop=0.0, attn_drop=0.0).cuda()
+    x = _rand((N, 32), 76)
+    e = _rand((E, 128), 77, scale=0.5).requires_grad_()
+    conv(g, x, e).square().sum().backward()          # warm: CSRs and workspaces built outside the profiled calls
+    calls = []
+    for name in ("pglb_dot_attn_e_csr_f32", "pglb_dot_attn_e_bwd_edge_f32", "pglb_dot_attn_csr_f32",
+                 "pglb_dot_attn_bwd_edge_f32"):
+        def spy(*a, _fn=getattr(ops.lib, name), _name=name):
+            rc = _fn(*a)
+            calls.append((_name, rc))
+            return rc
+        monkeypatch.setattr(ops.lib, name, spy)
+    fused = _kernels_of(lambda: conv(g, x, e).square().sum().backward())[0]
+    assert sorted(calls) == [("pglb_dot_attn_e_bwd_edge_f32", 0), ("pglb_dot_attn_e_csr_f32", 0)], calls
+    calls.clear()
+    opby = _kernels_of(lambda: _op_by_op(pgl, conv, g, x, e).square().sum().backward())[0]
+    assert calls == []
+    if not opby:
+        pytest.skip("torch.profiler records no CUDA kernels here")
+    assert len(fused) < len(opby), (len(fused), len(opby))
+
+
+def test_training_tracks_the_op_by_op_route(pgl, graph):
+    """A few Adam steps from one initialisation: the fused and op-by-op layers stay within tolerance."""
+    g, edges = graph
+    N, E = g.num_nodes, len(edges)
+    x = _rand((N, 32), 78)
+    e0 = _rand((E, 128), 79, scale=0.5)
+    y = torch.randint(0, 16, (N,), device="cuda", generator=torch.Generator("cuda").manual_seed(80))
+    outs = []
+    for fused in (True, False):
+        torch.manual_seed(7)
+        conv = pgl.nn.TransformerConv(32, 16, num_heads=8, feat_drop=0.0, attn_drop=0.0).cuda()
+        head = torch.nn.Linear(128, 16).cuda()
+        e = torch.nn.Parameter(e0.clone())
+        opt = torch.optim.Adam(list(conv.parameters()) + list(head.parameters()) + [e], lr=0.01)
+        for _ in range(5):
+            h = conv(g, x, e) if fused else _op_by_op(pgl, conv, g, x, e)
+            loss = torch.nn.functional.cross_entropy(head(h), y)
+            opt.zero_grad()
+            loss.backward()
+            opt.step()
+        with torch.no_grad():
+            outs.append((conv(g, x, e), e.detach().clone()))
+    assert rel_err(outs[0][0], outs[1][0]) <= 1e-3
+    assert rel_err(outs[0][1], outs[1][1]) <= 1e-3
+
+
+def test_layer_peak_memory(pgl):
+    """2M edges at 8 x 16 fp32: one [E, H*Dh] tensor is 1 GB.  The fused forward + backward peak above the resident
+    inputs (e included) is grad_e, two [E, H] float32 buffers and node-sized terms: <= 1.25 GB, and below half the
+    op-by-op route's."""
+    n, E = 20000, 2_000_000
+    edges = O.chung_lu_edges(n, E, exponent=0.8, seed=81)
+    g = pgl.Graph(edges=edges, num_nodes=n)
+    g.tensor()
+    conv = pgl.nn.TransformerConv(64, 16, num_heads=8, feat_drop=0.0, attn_drop=0.0).cuda()
+    x = _rand((n, 64), 82)
+    e = _rand((E, 128), 83, scale=0.5)
+
+    def peak(fn):
+        ee = e.clone().requires_grad_()
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        base = torch.cuda.memory_allocated()
+        fn(g, x, ee).square().sum().backward()
+        torch.cuda.synchronize()
+        return torch.cuda.max_memory_allocated() - base
+
+    g._fwd_csr(), g._bwd_csr()
+    peak(conv)   # warm: the workspace and CSR caches are resident, not part of the step
+    fused = peak(conv)
+    opby = peak(lambda gg, xx, ee: _op_by_op(pgl, conv, gg, xx, ee))
+    assert fused <= 1.25e9 and fused < 0.5 * opby, (fused, opby)
