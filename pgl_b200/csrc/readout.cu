@@ -437,10 +437,14 @@ __global__ void __launch_bounds__(256) topk_smem_kernel(const float *__restrict_
     }
 }
 
-// long path: sort (segment << 32 | ~key) ascending, stable, with the node id as the value
+// long path: sort (segment << 32 | ~key) ascending, stable, with the node id as the value.  Nodes outside
+// [indptr[0], indptr[B]) belong to no segment, as on the shared-memory path: those before take the low word 0 in
+// segment 0 and those after take 0xffffffff in segment B - 1 (no score maps there: ~key >= 0x007fffff, NaN ties and
+// loses on the node id), so every segment's members keep the sorted positions [indptr[g], indptr[g + 1]).
 __global__ void __launch_bounds__(256) topk_pack_kernel(const float *__restrict__ scores, int64_t N,
                                                         const int64_t *__restrict__ indptr, int64_t B,
                                                         uint64_t *__restrict__ keys, uint64_t *__restrict__ vals) {
+    const int64_t first = __ldg((const long long *)indptr), last = __ldg((const long long *)indptr + B);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += (int64_t)gridDim.x * blockDim.x) {
         int64_t lo = 0, hi = B;  // last g with indptr[g] <= i
         while (hi - lo > 1) {
@@ -448,7 +452,8 @@ __global__ void __launch_bounds__(256) topk_pack_kernel(const float *__restrict_
             if (__ldg((const long long *)indptr + mid) <= i) lo = mid;
             else hi = mid;
         }
-        keys[i] = ((uint64_t)lo << 32) | (uint64_t)(~topk_key(__ldg(scores + i)));
+        const uint32_t low = i < first ? 0u : i >= last ? 0xffffffffu : ~topk_key(__ldg(scores + i));
+        keys[i] = ((uint64_t)lo << 32) | (uint64_t)low;
         vals[i] = (uint64_t)i;
     }
 }
@@ -459,8 +464,8 @@ __global__ void __launch_bounds__(256) topk_emit_kernel(const uint64_t *__restri
                                                         const int64_t *__restrict__ off, int64_t *__restrict__ perm) {
     for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < N; p += (int64_t)gridDim.x * blockDim.x) {
         const int64_t g = (int64_t)(keys[p] >> 32);
-        const int64_t r = p - indptr[g];
-        if (r < off[g + 1] - off[g]) perm[off[g] + r] = (int64_t)vals[p];
+        const int64_t r = p - indptr[g];  // < 0 before indptr[0], >= the segment's length after indptr[B]
+        if (r >= 0 && r < off[g + 1] - off[g]) perm[off[g] + r] = (int64_t)vals[p];
     }
 }
 

@@ -312,6 +312,7 @@ def attn_readout(x, indptr, gate=None, query=None, return_lse=False):
 def segment_topk_perm(scores, indptr, ratio):
     """perm of segment_topk (reference pgl/math.py:342-359): for every segment g of indptr, the nodes of its first
     k_g ranks (score descending, -0.0 == +0.0, NaN last, ties by ascending node index), segments in order.
+    Scores outside [indptr[0], indptr[B]) belong to no segment and are never ranked, on either kernel path.
     k_g = ceil(fp32(ratio) * fp32(n_g)) for a float ratio in (0, 1], min(ratio, n_g) for an int ratio >= 1.  Scores
     are ranked in float32, as the reference's dense score matrix holds them.  One 16-byte read back (the total and the
     longest segment), as the reference also synchronises here."""
