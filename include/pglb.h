@@ -758,6 +758,57 @@ int pglb_metapath_walk_host(const int64_t *const *indptrs, const int64_t *const 
                             const int64_t *nodes, int64_t n, int64_t walk_length, uint64_t seed, int64_t *out);
 
 /* ------------------------------------------------------------------------------------
+ * Skip-gram pairs and alias-table sampling (csrc/skipgram.cu; alias build in csrc/host.cpp).  Replace the reference's
+ * graph_kernel.skip_gram_gen_pair (graph_kernel.pyx:343-365) called once per walk, and the host negative sampling of
+ * its walk examples (graph_kernel.alias_sample_build_table, graph_kernel.pyx:368-393, and alias_sample,
+ * examples/metapath2vec/datasets/sampling.py:133-146).
+ *
+ * Counter tags: the fourth Philox counter word of the two streams below.  The walk kernels put a trial number there,
+ * at most max(16, deg) for a row of deg slots, so no row shorter than 2^32 - 2 slots shares a counter with them. */
+#define PGLB_SKIPGRAM_TAG 0xFFFFFFFFu
+#define PGLB_ALIAS_TAG 0xFFFFFFFEu
+/* Skip-gram pairs.  walks: int64 [B, L] row-major, each row a walk padded with -1 (the walk entries' layout).
+ *   - Walk b has length n_b: the index of the first entry < 0 in its row, or L if there is none.
+ *   - Centre i < n_b has the window w = 1 + mulhi32(word0, win_size), in [1, win_size], where word0..3 =
+ *     Philox4x32-10(counter = (b lo32, b hi32, i, PGLB_SKIPGRAM_TAG), key = (seed lo32, seed hi32)).
+ *   - The centre emits (walk[b][i], walk[b][j]) for every j from max(0, i - w) to min(n_b - 1, i + w) ascending,
+ *     skipping each j with walk[b][j] == walk[b][i] (by node id, not position: a revisited node never pairs with
+ *     itself).  Output order: walk, then centre, then j -- the reference's per-walk outputs concatenated.  Given the
+ *     same windows the output is the reference's.
+ *   - win_size in [1, 2^31), L in [0, 2^31 - 1), B >= 0; a NULL pointer with B > 0: PGLB_EINVAL before any CUDA call.
+ *     B = 0 is a no-op (offsets is not written).  Pair offsets are int64; the total may exceed 2^32.
+ * pglb_skipgram_count: offsets[0..B] = exclusive scan of the per-walk pair counts, offsets[B] = total (B + 1 device
+ *   entries): one counting launch and the three launches of the multi-block int64 scan.  ws: device scratch of
+ *   pglb_skipgram_count_ws(B) bytes (too small: PGLB_EWORKSPACE).
+ * pglb_skipgram_fill: src[offsets[b] ..] / pos[offsets[b] ..] = the pairs of walk b (offsets from the count with the
+ *   same walks, win_size and seed); one launch, a warp per walk.
+ * pglb_skipgram_host: both over host arrays, blocking, by the kernels' own window and emit functions; src and pos may
+ *   both be NULL to count only.  For tests and small batches. */
+int pglb_skipgram_count_ws(int64_t B, size_t *ws_bytes);
+int pglb_skipgram_count(const int64_t *walks, int64_t B, int64_t L, int64_t win_size, uint64_t seed, int64_t *offsets,
+                        void *ws, size_t ws_bytes, void *stream);
+int pglb_skipgram_fill(const int64_t *walks, int64_t B, int64_t L, int64_t win_size, uint64_t seed,
+                       const int64_t *offsets, int64_t *src, int64_t *pos, void *stream);
+int pglb_skipgram_host(const int64_t *walks, int64_t B, int64_t L, int64_t win_size, uint64_t seed, int64_t *offsets,
+                       int64_t *src, int64_t *pos);
+/* Alias table build, on the host: graph_kernel.pyx:368-393 exactly -- alias = probs * n in float64, the indices with
+ * alias > 1 and < 1 on two stacks, and while both are non-empty: s = top of smaller (popped), l = top of larger,
+ * events[s] = l, alias[l] -= (1 - alias[s]), pop l if alias[l] <= 1, push l on smaller if alias[l] < 1.  Output
+ * equals the reference's bit for bit (compiled without FMA contraction), including the entries whose events stay 0
+ * after rounding.  probs is used as given (no normalisation).  n = 0: no-op; n < 0 or a NULL pointer: PGLB_EINVAL. */
+int pglb_alias_build_host(const double *probs, int64_t n, double *alias, int64_t *events);
+/* Alias sampling: out[k], k < count, is draw k of the table (alias float64 [n], events int64 [n]):
+ * word0..3 = Philox4x32-10(counter = (k lo32, k hi32, 0, PGLB_ALIAS_TAG), key = (seed lo32, seed hi32));
+ * slot = mulhi64(word1 << 32 | word0, n); u = ((word2 << 32 | word3) >> 11) * 2^-53; out[k] = slot if u < alias[slot],
+ * else events[slot] (the reference's alias_sample rule: uni >= alias[idx] takes the event).  n in [1, 2^32), count >= 0,
+ * NULL pointers with count > 0: PGLB_EINVAL before any CUDA call; count = 0 is a no-op.
+ * pglb_alias_sample: device arrays, one launch.  pglb_alias_sample_host: host arrays by the kernel's own draw. */
+int pglb_alias_sample(const double *alias, const int64_t *events, int64_t n, int64_t count, uint64_t seed,
+                      int64_t *out, void *stream);
+int pglb_alias_sample_host(const double *alias, const int64_t *events, int64_t n, int64_t count, uint64_t seed,
+                           int64_t *out);
+
+/* ------------------------------------------------------------------------------------
  * Graph-level readouts (csrc/readout.cu).  Every entry is keyed by a segment CSR indptr[B + 1] (device int64,
  * non-decreasing, indptr[0] = 0, indptr[B] = N): segment g is the contiguous rows indptr[g] .. indptr[g + 1] - 1 (a
  * batched graph's _graph_node_index).  Every output element has exactly one writer, there are no atomics, and the

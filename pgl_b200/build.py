@@ -63,7 +63,9 @@ def build_lib(force=False, verbose=False):
         objs.append(o)
         if not force and not _stale(o, [s] + hdrs):
             continue
-        cmd = ["nvcc"] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-c", s, "-o", o]
+        # host-only C++ (host.cpp: the alias table build) must round like the reference: no FMA contraction
+        host = ["-Xcompiler", "-ffp-contract=off"] if s.endswith(".cpp") else []
+        cmd = ["nvcc"] + NVCC_FLAGS + host + (["-Xptxas", "-v"] if verbose else []) + ["-c", s, "-o", o]
         procs.append((s, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT,
                                           text=True)))
     for s, p in procs:

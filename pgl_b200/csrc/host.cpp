@@ -1,6 +1,7 @@
 // host.cpp -- host-side entry points of libpglb: error reporting, the numpy-mode CSR build
 // (twin of pgl/graph_kernel.pyx:59-88) and the METIS K-way wrapper
-// (pgl/graph_kernel.pyx:434-472), which dlopen()s a libmetis built with IDXTYPEWIDTH=64.
+// (pgl/graph_kernel.pyx:434-472), which dlopen()s a libmetis built with IDXTYPEWIDTH=64, and the alias table build
+// (pgl/graph_kernel.pyx:368-393).
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <stdarg.h>
@@ -76,6 +77,35 @@ extern "C" int pglb_memcpy2d_async(void *dst, size_t dst_pitch, const void *src,
                                       kind == 1 ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToHost,
                                       reinterpret_cast<cudaStream_t>(stream));
     if (e != cudaSuccess) return cuda_fail(e, "cudaMemcpy2DAsync");
+    return PGLB_OK;
+}
+
+// ---- alias table (graph_kernel.pyx:368-393) ------------------------------------------------------
+// Vose's construction as the reference runs it: alias = probs * n in float64, the indices above and below 1 on two
+// stacks, and each step pairs the top of both.  Built without FMA contraction (pgl_b200/build.py), so every value is
+// the reference's bit for bit, its rounding leftovers (entries whose events stay 0) included.
+extern "C" int pglb_alias_build_host(const double *probs, int64_t n, double *alias, int64_t *events) {
+    if (n < 0) return fail(PGLB_EINVAL, "pglb_alias_build_host: negative n");
+    if (n == 0) return PGLB_OK;
+    if (!probs || !alias || !events) return fail(PGLB_EINVAL, "pglb_alias_build_host: NULL pointer");
+    const double dn = (double)n;
+    std::vector<int64_t> larger, smaller;
+    for (int64_t i = 0; i < n; ++i) {
+        alias[i] = probs[i] * dn;
+        events[i] = 0;
+    }
+    for (int64_t i = 0; i < n; ++i) {
+        if (alias[i] > 1) larger.push_back(i);
+        else if (alias[i] < 1) smaller.push_back(i);
+    }
+    while (!smaller.empty() && !larger.empty()) {
+        const int64_t s = smaller.back(), l = larger.back();
+        smaller.pop_back();
+        events[s] = l;
+        alias[l] -= (1 - alias[s]);
+        if (alias[l] <= 1) larger.pop_back();
+        if (alias[l] < 1) smaller.push_back(l);
+    }
     return PGLB_OK;
 }
 

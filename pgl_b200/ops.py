@@ -217,6 +217,47 @@ def metapath_walk(indptrs, cols_list, num_nodes, nodes, walk_length, seed):
     return out
 
 
+# skip-gram pairs and alias sampling (csrc/skipgram.cu)
+# ------------------------------------------------------------------------------------------
+
+
+def skip_gram_pairs(walks, win_size, seed):
+    """pglb_skipgram_count + pglb_skipgram_fill: (src, pos) int64 pairs of the padded [B, L] int64 walks.  One count,
+    the scan, one device-to-host read of the total and one fill."""
+    require_cuda(walks)
+    walks = _i64(walks).contiguous()
+    B, L = walks.shape
+    dev = walks.device
+    if B == 0 or L == 0:
+        return (torch.empty(0, dtype=torch.int64, device=dev), torch.empty(0, dtype=torch.int64, device=dev))
+    offsets = torch.empty(B + 1, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        need = ctypes.c_size_t(0)
+        check(lib.pglb_skipgram_count_ws(B, ctypes.byref(need)))
+        ws = workspace(dev, need.value)
+        check(lib.pglb_skipgram_count(_ptr(walks), B, L, int(win_size), int(seed), _ptr(offsets), _ptr(ws),
+                                      ws.numel(), _stream()))
+        total = int(offsets[B].item())
+        src = torch.empty(total, dtype=torch.int64, device=dev)
+        pos = torch.empty(total, dtype=torch.int64, device=dev)
+        if total:
+            check(lib.pglb_skipgram_fill(_ptr(walks), B, L, int(win_size), int(seed), _ptr(offsets), _ptr(src),
+                                         _ptr(pos), _stream()))
+    return src, pos
+
+
+def alias_sample(alias, events, count, seed):
+    """pglb_alias_sample: count int64 draws of the table (alias float64 [n], events int64 [n]) on their device."""
+    require_cuda(alias, events)
+    alias = alias.to(torch.float64).contiguous()
+    events = _i64(events).contiguous()
+    out = torch.empty(int(count), dtype=torch.int64, device=alias.device)
+    with torch.cuda.device(alias.device):
+        check(lib.pglb_alias_sample(_ptr(alias), _ptr(events), alias.numel(), int(count), int(seed), _ptr(out),
+                                    _stream()))
+    return out
+
+
 # graph-level readouts (csrc/readout.cu)
 # ------------------------------------------------------------------------------------------
 
