@@ -6,7 +6,7 @@
 //   mode 0  LDG.128 per lane per row, 8 rows in flight per lane (registers)
 //   mode 1  cp.async.bulk (UBLKCP) 512 B per row from an elected lane, mbarrier per group of GR rows
 //   mode 2  cp.async.bulk 512 B per row from the lane that holds the row id (spmm_v5's mechanism)
-//   mode 3  LDGSTS per lane per row (cp.async.cg 16 B), commit groups of 4 (PGLB_STREAM_V5=2)
+//   mode 3  LDGSTS per lane per row (cp.async.cg 16 B), commit groups of 4
 //   mode 4  hybrid: a row whose id has bit 31 set is fetched by all 32 lanes (cp.async.cg 16 B, L2 evict_last) into
 //           its ring slot, every other row by mode 2's bulk copy (evict_first); the mbarrier expects only the bulk bytes
 // Every warp reduces chunks of T indices; the sum is written once per chunk (keeps the loads live).

@@ -864,14 +864,6 @@ int pglb_segment_pad(const void *x, int64_t num_rows, int64_t dim, int elem_size
 int pglb_segment_unpad(const void *padded, int64_t num_segments, int64_t max_len, int64_t dim, int elem_size,
                        const int64_t *indptr, int64_t num_rows, void *out, void *stream);
 
-/* Same contract as pglb_memcpy2d_async, but the copy is done by a kernel through the unified address
- * space (zero-copy loads / stores across PCIe; the host side must be pinned memory).  For narrow column
- * blocks, where the copy engine's 2-D transfers run at about half the PCIe rate.  width, pitches and both
- * pointers multiples of 16 bytes; ctas <= 0 -> 16.  Opt-in (PGLB_HOST_COPY=kernel) and unmeasured: the cross-call
- * pipeline of Graph.host_aggregator removed the need for narrow 2-D copies (DESIGN.md section 4.7). */
-int pglb_copy2d_kernel_async(void *dst, size_t dpitch, const void *src, size_t spitch, size_t width_bytes,
-                             int64_t height, int ctas, void *stream);
-
 /* norm[i] = clip(float(degree[i]), 1)^-0.5 ; GF.degree_norm (graph_op.py:46-55) */
 int pglb_degree_norm_f32(const int64_t *degree, int64_t n, float *norm, void *stream);
 

@@ -103,7 +103,6 @@ _SIGS = {
     "pglb_segment_topk_fill": (c_int, [_p, _i64, _p, _i64, _p, _i64, _p, _p, c_size_t, _p]),
     "pglb_segment_pad": (c_int, [_p, _i64, _i64, c_int, _p, _i64, _i64, _u64, _p, _p]),
     "pglb_segment_unpad": (c_int, [_p, _i64, _i64, _i64, c_int, _p, _i64, _p, _p]),
-    "pglb_copy2d_kernel_async": (c_int, [_p, c_size_t, _p, c_size_t, c_size_t, _i64, c_int, _p]),
     "pglb_linear_tf32x3_f32": (c_int, [_p, _i64, _p, _p, _p, _i64, _i64, _i64, _i64, c_int, _p]),
     "pglb_gat_fused_csr_f32": (c_int, [_p, _p, _p, _i64, _p, _p, ctypes.c_float, _p, _i64, _i64, _i64, _i64,
                                        _i64, _i64, _p, c_size_t, _p]),

@@ -10,8 +10,6 @@
 // ReLU it replaces moved 20.5 GB and ran on the CUDA cores).
 //
 // K = N = 128 goes to the wgmma kernel of linear_wgmma.cu; this kernel takes every other shape.
-#include <stdlib.h>
-
 #include <algorithm>
 
 #include "common.cuh"
@@ -19,7 +17,7 @@
 namespace pglb {
 
 constexpr int LT_ROWS = 64;        // rows of x per tile: 4 row blocks of 16
-constexpr int LT_WARPS_DEFAULT = 8;  // 8 warps = 4 row blocks x 2 column groups; 16 = 4 x 4
+constexpr int LT_WARPS = 8;  // 4 row blocks x 2 column groups
 constexpr int LT_KMAX = 128;
 constexpr int LT_XS = LT_KMAX + 4;  // x tile row stride (floats): 132 = 4 mod 32 -> conflict-free A loads
 
@@ -32,14 +30,14 @@ __device__ __forceinline__ void cp_async16_zfill(void *smem, const void *gmem, i
 // N = output width (64 or 128).  Dynamic shared memory:
 //   W2 [LT_KMAX][N + 4] of {hi, lo} tf32 pairs (rows >= K are zero)
 //   X  [2][LT_ROWS][LT_XS] fp32 (columns >= K stay zero)
-template <int N, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32, 1)
+template <int N>
+__global__ void __launch_bounds__(LT_WARPS * 32, 1)
 linear_tf32x3_kernel(const float *__restrict__ x, int64_t ldx, const float *__restrict__ w,
                      const float *__restrict__ bias, float *__restrict__ out, int64_t ldo, int64_t M,
                      int K, int act) {
     constexpr int WS = N + 4;    // W2 row stride in pairs: (N+4) = 4 mod 16 -> conflict-free LDS.64
-    constexpr int LT_THREADS = WARPS * 32;
-    constexpr int CG = WARPS / 4;    // column groups
+    constexpr int LT_THREADS = LT_WARPS * 32;
+    constexpr int CG = LT_WARPS / 4;    // column groups
     constexpr int WCOLS = N / CG;    // columns owned by one warp
     constexpr int NT = WCOLS / 8;    // 8-wide column tiles per warp
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -152,15 +150,15 @@ linear_tf32x3_kernel(const float *__restrict__ x, int64_t ldx, const float *__re
     }
 }
 
-template <int N, int WARPS>
+template <int N>
 static int launch(const float *x, int64_t ldx, const float *w, const float *bias, float *out,
                   int64_t ldo, int64_t M, int K, int act, cudaStream_t stream) {
     const size_t smem = sizeof(uint2) * LT_KMAX * (N + 4) + sizeof(float) * 2 * LT_ROWS * LT_XS;
     static std::atomic<unsigned long long> attr_done{0};
-    PGLB_CUDA(ensure_dyn_smem(linear_tf32x3_kernel<N, WARPS>, (int)smem, attr_done));
+    PGLB_CUDA(ensure_dyn_smem(linear_tf32x3_kernel<N>, (int)smem, attr_done));
     const int64_t tiles = (M + LT_ROWS - 1) / LT_ROWS;
     const unsigned grid = (unsigned)std::min<int64_t>(tiles, sm_count());
-    linear_tf32x3_kernel<N, WARPS><<<grid, WARPS * 32, smem, stream>>>(x, ldx, w, bias, out, ldo, M, K, act);
+    linear_tf32x3_kernel<N><<<grid, LT_WARPS * 32, smem, stream>>>(x, ldx, w, bias, out, ldo, M, K, act);
     PGLB_LAUNCH_CHECK("linear_tf32x3_kernel");
     return PGLB_OK;
 }
@@ -168,7 +166,6 @@ static int launch(const float *x, int64_t ldx, const float *w, const float *bias
 }  // namespace pglb
 
 namespace pglb {
-bool linear_wgmma_enabled();
 int linear_wgmma_run(const float *x, int64_t ldx, const float *w, const float *bias, float *out, int64_t ldo,
                      int64_t M, int act, cudaStream_t stream);
 }  // namespace pglb
@@ -191,17 +188,7 @@ extern "C" int pglb_linear_tf32x3_f32(const float *x, int64_t ldx, const float *
                    "pglb_linear_tf32x3_f32: x must be 16-byte and out 8-byte aligned");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     // K = N = 128 (the conv layers' hidden size): wgmma / TMA kernel (csrc/linear_wgmma.cu)
-    if (K == 128 && N == 128 && linear_wgmma_enabled())
-        return linear_wgmma_run(x, ldx, w, bias, out, ldo, M, act, s);
-    // PGLB_LINEAR_WARPS = 8 | 16 picks the CTA shape (tuning knob; both are covered by the tests)
-    int warps = LT_WARPS_DEFAULT;
-    if (const char *e = getenv("PGLB_LINEAR_WARPS")) {
-        const int v = atoi(e);
-        if (v == 8 || v == 16) warps = v;
-    }
-    if (N == 128)
-        return warps == 16 ? launch<128, 16>(x, ldx, w, bias, out, ldo, M, (int)K, act, s)
-                           : launch<128, 8>(x, ldx, w, bias, out, ldo, M, (int)K, act, s);
-    return warps == 16 ? launch<64, 16>(x, ldx, w, bias, out, ldo, M, (int)K, act, s)
-                       : launch<64, 8>(x, ldx, w, bias, out, ldo, M, (int)K, act, s);
+    if (K == 128 && N == 128) return linear_wgmma_run(x, ldx, w, bias, out, ldo, M, act, s);
+    if (N == 128) return launch<128>(x, ldx, w, bias, out, ldo, M, (int)K, act, s);
+    return launch<64>(x, ldx, w, bias, out, ldo, M, (int)K, act, s);
 }

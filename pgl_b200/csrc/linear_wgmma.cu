@@ -13,8 +13,6 @@
 // every 128-row tile.  Shared memory: W^T hi / lo (128 KB), STAGES x (raw + lo) K blocks of the x tile (32 KB each).
 #include <cuda.h>
 
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace pglb {
@@ -239,16 +237,6 @@ typedef CUresult (*TmapEncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t,
                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 }  // namespace wg
-
-// PGLB_LINEAR_WGMMA = 0 keeps every shape on the mma.sync kernel (linear_tc.cu)
-bool linear_wgmma_enabled() {
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("PGLB_LINEAR_WGMMA");
-        v = (e && atoi(e) == 0) ? 0 : 1;
-    }
-    return v == 1;
-}
 
 // K = N = 128, x rows 16-byte aligned (ldx % 4 == 0), out 8-byte aligned with even ldo: checked by the caller
 int linear_wgmma_run(const float *x, int64_t ldx, const float *w, const float *bias, float *out, int64_t ldo,

@@ -64,10 +64,10 @@ struct StreamP {
     float slope;             // YM 2: LeakyReLU negative slope
     float *partial_ml;       // YM 2: [2*ntasks, 64] running (max, sum) of cut rows, per lane
     int accumulate;          // SUM only: out = (out_prev + sum) * scale_dst
-    unsigned *counter;       // task queue head of the persistent (DYN) kernels, zeroed by task_plan_kernel
+    unsigned *counter;       // task queue head of the persistent kernels, zeroed by task_plan_kernel
     long long *trace;        // debug, nullable: [ntasks, 4] = (start ns, end ns, SM id, warp slot) per task (pglb_debug_task_trace)
     float *lse;              // YM 2, nullable: [n_rows, H] log-sum-exp of every non-empty row's logits (saved for backward)
-    int dyn;                 // 0: static block -> task map, 1: dynamic ascending, 2: dynamic descending
+    int dyn;                 // task order of the queue: 1 ascending, 2 descending
 };
 
 __device__ __forceinline__ void cp_async16(unsigned smem_dst, const void *gsrc) {
@@ -261,21 +261,15 @@ __global__ void __launch_bounds__(Geo<YM>::kWarps * 32, 2) spmm_stream128_kernel
     const char *xlane = reinterpret_cast<const char *>(p.x) + (act ? lane * 16 : 0);
     const unsigned row_bytes = (unsigned)(p.ldx * 4);
 
-    // p.dyn != 0: persistent warps draw task ids from the device-side queue (see spmm_v5_kernel); the per-lane
-    // cp.async rings are drained at the end of every task, so a task starts from a clean ring either way
+    // persistent warps draw task ids from the device-side queue (see spmm_v5_kernel); the per-lane cp.async rings are
+    // drained at the end of every task, so a task starts from a clean ring
 #pragma unroll 1
     for (;;) {
-    int64_t task;
-    if (p.dyn) {
-        unsigned t = 0;
-        if (lane == 0) t = atomicAdd(p.counter, 1u);
-        t = __shfl_sync(0xffffffffu, t, 0);
-        if ((int64_t)t >= p.ntasks) break;
-        task = p.dyn == 2 ? p.ntasks - 1 - (int64_t)t : (int64_t)t;
-    } else {
-        task = (int64_t)blockIdx.x * W + wib;
-        if (task >= p.ntasks) break;
-    }
+    unsigned t = 0;
+    if (lane == 0) t = atomicAdd(p.counter, 1u);
+    t = __shfl_sync(0xffffffffu, t, 0);
+    if ((int64_t)t >= p.ntasks) break;
+    const int64_t task = p.dyn == 2 ? p.ntasks - 1 - (int64_t)t : (int64_t)t;
     m_run = -INFINITY;
     l_run = 0.0f;
     ad = 0.0f;
@@ -505,7 +499,6 @@ __global__ void __launch_bounds__(Geo<YM>::kWarps * 32, 2) spmm_stream128_kernel
         }
     }
     if (lane == 0) p.tail_row[task] = tail;
-    if (!p.dyn) break;
     cp_async_wait<0>();   // nothing real is pending; keeps the group count of the next task's pipeline exact
     }
 }
@@ -923,18 +916,11 @@ static int64_t gat_task_size(int64_t E) {
 // one workspace size for every kernel of the family: the layout of the smallest task size any of them uses
 size_t stream_ws_bytes(int64_t E, int64_t D) { return stream_layout(nullptr, E, D, gat_task_size(E)).bytes; }
 
-// Task hand-out of the persistent kernels (spmm_v5 / spmm_gat5): 0 = static block -> task map, 1 = device-side queue
-// in ascending task order, 2 = queue in descending order.  slot 0: PGLB_V5_DYN, slot 1: PGLB_GAT_DYN (read per
-// call -- a getenv, no cache -- so one process can compare the modes).
-// Defaults: the copy-sum kernel takes the queue in ascending order when there are many tasks per resident warp and in
-// descending order when there are few.  The fused GAT kernel takes the DESCENDING queue: RMAT puts the expensive tasks
+// Task order of the persistent kernels' device-side queue (StreamP::dyn): 1 = ascending, 2 = descending.  slot 0: the
+// copy-sum kernel (spmm_v5), which takes ascending order when there are many tasks per resident warp and descending
+// order when there are few.  Every other kernel (slot >= 1) takes descending order: RMAT puts the expensive tasks
 // (one-edge rows) last, the descending queue starts them first and every warp stays busy to the end of the launch.
-static int dyn_mode(const char *name, int slot, int64_t ntasks) {
-    const char *e = getenv(name);
-    if (e) {
-        const int v = atoi(e);
-        if (v >= 0 && v <= 2) return v;
-    }
+static int dyn_mode(int slot, int64_t ntasks) {
     if (slot >= 1) return 2;
     const int64_t resident_warps = (int64_t)sm_count() * 2 * 13;
     return ntasks >= 8 * resident_warps ? 1 : 2;
@@ -957,7 +943,7 @@ static int launch_stream128(const StreamP &p, cudaStream_t stream) {
     PGLB_CUDA(ensure_dyn_smem(spmm_stream128_kernel<RK, SCALED, PK, YM>, smem, attr_done));
     int64_t blocks = (p.ntasks + W - 1) / W;
     PGLB_CHECK_ARG(blocks <= 0x7fffffffLL, PGLB_ESHAPE, "spmm_stream: grid too large");
-    if (p.dyn && blocks > (int64_t)sm_count() * 2) blocks = (int64_t)sm_count() * 2;   // persistent: 2 CTAs per SM
+    if (blocks > (int64_t)sm_count() * 2) blocks = (int64_t)sm_count() * 2;   // persistent: 2 CTAs per SM
     spmm_stream128_kernel<RK, SCALED, PK, YM><<<(unsigned)blocks, W * 32, smem, stream>>>(p);
     PGLB_LAUNCH_CHECK("spmm_stream128_kernel");
     const int64_t fblocks = (p.ntasks * 32 + 255) / 256;
@@ -988,7 +974,7 @@ static int launch_stream(const StreamP &p, int tiles, cudaStream_t stream) {
 }
 
 // Task plan and launch parameters shared by the wide-row runs below: fills everything of p but the edge operand,
-// accumulate and the task hand-out p.dyn (left to the caller), and launches task_plan_kernel for tasks of T slots.
+// accumulate and the queue order p.dyn (left to the caller), and launches task_plan_kernel for tasks of T slots.
 // `ws` holds >= stream_ws_bytes().
 static int stream_prepare(StreamP &p, int64_t T, const int64_t *indptr, const int64_t *cols, const void *x, int64_t ldx,
                           void *out, int64_t ldo, int64_t n_dst, int64_t E, int64_t D, int reduce_op,
@@ -1046,7 +1032,7 @@ int spmm_v5_run(const int64_t *indptr, const int64_t *cols, const void *x, int64
                                       scale_src, scale_slot, scale_dst, cols32, ws, ws_bytes, stream);
         if (rc) return rc;
     }
-    p.dyn = dyn_mode("PGLB_V5_DYN", 0, p.ntasks);
+    p.dyn = dyn_mode(0, p.ntasks);
     {
         const int rc = launch_empty_rows<T>(p, stream);
         if (rc) return rc;
@@ -1077,7 +1063,7 @@ int gatv2_attn_run(const int64_t *indptr, const int64_t *cols, const void *f, in
                                       PGLB_REDUCE_SUM, nullptr, nullptr, nullptr, nullptr, ws, ws_bytes, stream);
         if (rc) return rc;
     }
-    p.dyn = dyn_mode("PGLB_GAT_DYN", 1, p.ntasks);
+    p.dyn = dyn_mode(1, p.ntasks);
     {
         const int rc = launch_empty_rows<T>(p, stream);
         if (rc) return rc;
@@ -1121,7 +1107,7 @@ int spmm_stream_run(const int64_t *indptr, const int64_t *cols, const float *x, 
                                       scale_src, nullptr, scale_dst, cols32, ws, ws_bytes, stream);
         if (rc) return rc;
     }
-    p.dyn = dyn_mode("PGLB_S128_DYN", 2, p.ntasks);   // round 1's kernel (max / min, edge operands): descending queue
+    p.dyn = dyn_mode(2, p.ntasks);   // round 1's kernel (max / min, edge operands): descending queue
     {
         const int rc = launch_empty_rows<float>(p, stream);
         if (rc) return rc;
@@ -1273,7 +1259,7 @@ int gat_fused_run(const int64_t *indptr, const int64_t *cols, const void *f, int
                                       nullptr, nullptr, nullptr, nullptr, ws, ws_bytes, stream);
         if (rc) return rc;
     }
-    p.dyn = dyn_mode("PGLB_GAT_DYN", 1, p.ntasks);
+    p.dyn = dyn_mode(1, p.ntasks);
     {
         const int rc = launch_empty_rows<T>(p, stream);
         if (rc) return rc;
@@ -1310,7 +1296,7 @@ int dot_attn_run(const int64_t *indptr, const int64_t *cols, const void *q, int6
                                       PGLB_REDUCE_SUM, nullptr, nullptr, nullptr, nullptr, ws, ws_bytes, stream);
         if (rc) return rc;
     }
-    p.dyn = dyn_mode("PGLB_GAT_DYN", 1, p.ntasks);
+    p.dyn = dyn_mode(1, p.ntasks);
     {
         const int rc = launch_empty_rows<T>(p, stream);
         if (rc) return rc;

@@ -669,20 +669,10 @@ def _spmm_raw(indptr, cols, x2, n_dst, reduce_op, eid=None, y2=None, y_bcast=BCA
     return out
 
 
-# PGLB_HOST_COPY=kernel (experimental): move the column blocks of HostAggregator with a zero-copy kernel
-# instead of cudaMemcpy2DAsync (csrc/host_copy.cu); PGLB_HOST_COPY_CTAS sets its grid (default 16)
-HOST_COPY_KERNEL = os.environ.get("PGLB_HOST_COPY") == "kernel"
-HOST_COPY_CTAS = int(os.environ.get("PGLB_HOST_COPY_CTAS", "16"))
-
-
 def _copy2d(dst_ptr, dpitch, src_ptr, spitch, width, height, kind, stream):
     """kind 1: host -> device, 2: device -> host (pglb_memcpy2d_async's convention)."""
-    if HOST_COPY_KERNEL:
-        check(lib.pglb_copy2d_kernel_async(ctypes.c_void_p(dst_ptr), dpitch, ctypes.c_void_p(src_ptr), spitch,
-                                           width, height, HOST_COPY_CTAS, ctypes.c_void_p(stream)))
-    else:
-        check(lib.pglb_memcpy2d_async(ctypes.c_void_p(dst_ptr), dpitch, ctypes.c_void_p(src_ptr), spitch,
-                                      width, height, kind, ctypes.c_void_p(stream)))
+    check(lib.pglb_memcpy2d_async(ctypes.c_void_p(dst_ptr), dpitch, ctypes.c_void_p(src_ptr), spitch,
+                                  width, height, kind, ctypes.c_void_p(stream)))
 
 
 class HostAggregator(object):
@@ -2222,14 +2212,9 @@ def launch_count():
 
 
 def stream_kernel_name(num_edges=None, num_rows=None):
-    """Which wide-row streaming kernel pglb_spmm_csr_f32 routes copy-sum aggregations to (PGLB_STREAM_V5, PGLB_V5_GEO,
-    PGLB_V5_DYN; mirrors csrc/spmm_v5.inl v5_mode() / v5_geo(): without PGLB_V5_GEO, graphs of >= 12 slots per row
-    take the groups-of-8 geometry)."""
-    v = os.environ.get("PGLB_STREAM_V5", "1")
-    g = os.environ.get("PGLB_V5_GEO")
-    if g not in ("0", "2"):
-        g = "2" if (num_edges is not None and num_rows and num_edges >= 12 * num_rows) else "0"
-    geo = {"0": "GRP=4,NG=4,W=13", "2": "GRP=8,NG=3,W=9"}[g]
-    how = "bulk copy per row (cp.async.bulk)" if v != "2" else "LDGSTS ring"
-    q = "" if os.environ.get("PGLB_V5_DYN") == "0" or v == "2" else ", device-side task queue"
-    return "spmm_v5_kernel<%s, %s%s> (+ task_plan, empty_rows, fix-up kernels)" % (how, geo, q)
+    """Which wide-row streaming kernel pglb_spmm_csr_f32 routes copy-sum aggregations to (mirrors csrc/spmm_v5.inl
+    v5_geo(): graphs of >= 12 slots per row take the groups-of-8 geometry)."""
+    wide = num_edges is not None and num_rows and num_edges >= 12 * num_rows
+    geo = "GRP=8,NG=3,W=9" if wide else "GRP=4,NG=4,W=13"
+    return ("spmm_v5_kernel<bulk copy per row (cp.async.bulk), %s, device-side task queue> (+ task_plan, empty_rows, "
+            "fix-up kernels)" % geo)

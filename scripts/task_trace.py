@@ -1,5 +1,5 @@
 """Per-task timeline of the fused GAT aggregation on cfg3 (pglb_debug_task_trace): where the launch's time goes by task
-id, how many warps are busy over time, the longest tasks.  One JSON line per task-queue mode."""
+id, how many warps are busy over time, the longest tasks.  One JSON line."""
 import json
 import os
 import sys
@@ -56,25 +56,23 @@ def main():
         f = (x @ conv.linear.weight + conv.linear.bias).reshape(-1, H, Dh).contiguous()
         a_s = (f * conv.weight_src).sum(-1).contiguous()
         a_d = (f * conv.weight_dst).sum(-1).contiguous()
-        for mode in (0, 1, 2):
-            os.environ["PGLB_GAT_DYN"] = str(mode)
-            for _ in range(3):
-                ops.gat_fused(csr, f, a_s, a_d, 0.2)
-            torch.cuda.synchronize()
-            ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            ev0.record()
-            for _ in range(10):
-                ops.gat_fused(csr, f, a_s, a_d, 0.2)
-            ev1.record()
-            torch.cuda.synchronize()
-            ms = ev0.elapsed_time(ev1) / 10
-            buf.zero_()
-            check(lib.pglb_debug_task_trace(ops._ptr(buf), cap))
+        for _ in range(3):
             ops.gat_fused(csr, f, a_s, a_d, 0.2)
-            torch.cuda.synchronize()
-            check(lib.pglb_debug_task_trace(None, 0))
-            analyse(buf.cpu().numpy(), "cfg3 fused GAT", {"dyn": mode, "ms_untraced": round(ms, 3),
-                                                          "task_env": os.environ.get("PGLB_STREAM_TASK", "default")})
+        torch.cuda.synchronize()
+        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        ev0.record()
+        for _ in range(10):
+            ops.gat_fused(csr, f, a_s, a_d, 0.2)
+        ev1.record()
+        torch.cuda.synchronize()
+        ms = ev0.elapsed_time(ev1) / 10
+        buf.zero_()
+        check(lib.pglb_debug_task_trace(ops._ptr(buf), cap))
+        ops.gat_fused(csr, f, a_s, a_d, 0.2)
+        torch.cuda.synchronize()
+        check(lib.pglb_debug_task_trace(None, 0))
+        analyse(buf.cpu().numpy(), "cfg3 fused GAT", {"ms_untraced": round(ms, 3),
+                                                      "task_env": os.environ.get("PGLB_STREAM_TASK", "default")})
 
 
 if __name__ == "__main__":

@@ -15,8 +15,7 @@ not exact in this sense and are tested elsewhere.
 
 Route coverage: `test_route_coverage` records the kernels each representative call launches (torch.profiler) and
 asserts that every route of the wide/narrow/generic families was reached and that each call hit the family it claims.
-Switches the library reads once per process (task size, copy mechanism, ring geometry) run the numeric tests again in
-child processes."""
+The task size, which the library reads once per process, runs the numeric tests again in child processes."""
 import os
 import re
 import subprocess
@@ -354,12 +353,9 @@ F32_WIDTHS = [1, 3, 4, 5, 8, 9, 16, 17, 20, 32, 33, 36, 64, 65, 68, 100, 124, 12
 X16_WIDTHS = [(torch.bfloat16, d) for d in (1, 3, 4, 5, 8, 9, 16, 17, 32, 33, 64, 65, 68, 72, 120, 128, 129, 132,
                                             257, 513, 516, 1024, 1433)] + \
              [(torch.float16, d) for d in (17, 72, 128, 132, 516)]
-if CHILD and "PGLB_STREAM_TASK" in os.environ:   # the widths of the kernels that cut rows into tasks
+if CHILD:                                         # the widths of the kernels that cut rows into tasks
     F32_WIDTHS = [36, 128, 260, 1024]
     X16_WIDTHS = [(torch.bfloat16, 128)]
-elif CHILD:                                       # the copy mechanism and ring geometry of spmm_v5_kernel
-    F32_WIDTHS = [100, 128]
-    X16_WIDTHS = [(torch.bfloat16, 72)]
 V5_F32 = (68, 100, 124, 128)
 V5_X16 = (72, 120, 128)
 COPY_CASES = [(torch.float32, d) for d in F32_WIDTHS] + X16_WIDTHS
@@ -591,18 +587,55 @@ def test_host_aggregator_column_blocks_exact(dim, chunks):
             assert_bits(got, want, "host aggregator dim=%d %s scaled=%s" % (dim, reduce_op, scaled), dst)
 
 
+def _queue_order(run, ntasks):
+    """'ascending' or 'descending': the order in which spmm_v5_kernel's device-side queue handed out the tasks of the
+    one launch `run` makes, read from the per-task start times of pglb_debug_task_trace.  With several waves of tasks
+    per resident warp the tasks handed out first start first."""
+    from pgl_b200 import ops
+    from pgl_b200._lib import check, lib
+    buf = torch.zeros((ntasks, 4), dtype=torch.int64, device="cuda")
+    torch.cuda.synchronize()
+    check(lib.pglb_debug_task_trace(ops._ptr(buf), ntasks))
+    try:
+        run()
+        torch.cuda.synchronize()
+    finally:
+        check(lib.pglb_debug_task_trace(None, 0))
+    start = buf[:, 0].cpu().numpy()
+    assert (start > 0).all(), "%d of %d tasks not traced" % (int((start <= 0).sum()), ntasks)
+    k = ntasks // 8
+    return "ascending" if np.median(start[:k]) < np.median(start[-k:]) else "descending"
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("var", ["PGLB_V5_DYN", "PGLB_S128_DYN"])
-@pytest.mark.parametrize("mode", ["0", "1", "2"])
-def test_task_handout_modes(monkeypatch, var, mode):
-    """Static, ascending-queue and descending-queue task hand-out of the wide-row kernels (read on every call)."""
-    monkeypatch.setenv(var, mode)
-    if var == "PGLB_V5_DYN":
-        for dtype, D in ((torch.float32, 128), (torch.float32, 100), (torch.bfloat16, 128)):
-            _run_copy_matrix(dtype, D, ("ladder", "chunglu"))
-    else:
-        _run_copy_matrix(torch.float32, 128, ("ladder", "chunglu"))
-        test_ue_exact(128, "head")
+def test_v5_queue_orders_exact():
+    """At 64 slots per task: a graph of 3 tasks per resident warp takes spmm_v5_kernel's descending queue and one of
+    more than 8 takes the ascending queue (dyn_mode in csrc/spmm_stream.cu).  Both orders, read from the task trace,
+    give the exact sums, means and scaled sums of rows cut into many tasks."""
+    if os.environ.get("PGLB_STREAM_TASK") != "64":
+        pytest.skip("runs in the PGLB_STREAM_TASK=64 child")
+    import pgl_b200 as pgl
+    T, n = 64, 100_000
+    resident_warps = torch.cuda.get_device_properties(0).multi_processor_count * 2 * 13
+    for order, tasks in (("descending", 3 * resident_warps), ("ascending", 9 * resident_warps)):
+        edges = O.chung_lu_edges(n, tasks * T, exponent=0.8, seed=tasks)
+        src, dst = edges[:, 0], edges[:, 1]
+        g = pgl.Graph(edges=edges, num_nodes=n)
+        g.tensor()
+        rng = np.random.default_rng(tasks)
+        ss, sd = _pow2(rng, n), _pow2(rng, n)
+        ss_d, sd_d = _dev(ss), _dev(sd)
+        for dtype, D, reduce_op, scaled in ((torch.float32, 128, "sum", True), (torch.float32, 100, "mean", False),
+                                            (torch.bfloat16, 128, "sum", False)):
+            x = _int_features(rng, n, D, dtype)
+            xd = _dev(x, dtype)
+            kw = dict(scale_src=ss_d, scale_dst=sd_d) if scaled else {}
+            want = copy_case(x, src, dst, n, reduce_op, dtype, **(dict(scale_src=ss, scale_dst=sd) if scaled else {}))
+            tag = "%s queue, %d tasks: %s D=%d %s scaled=%s" % (order, tasks, dtype, D, reduce_op, scaled)
+            got = {}
+            seen = _queue_order(lambda: got.setdefault("out", g._send_u_recv(xd, reduce_op, None, **kw)), tasks)
+            assert seen == order, "%s: the trace shows the %s order" % (tag, seen)
+            assert_bits(got["out"].cpu(), want, tag, dst)
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -754,19 +787,20 @@ def test_feature_matrix_over_4gib_exact():
 # switches read once per process: child processes
 # ----------------------------------------------------------------------------------------------------------------
 
-CHILD_ENVS = [{"PGLB_STREAM_TASK": "64"}, {"PGLB_STREAM_TASK": "2048"}, {"PGLB_STREAM_V5": "2"},
-              {"PGLB_V5_GEO": "0"}, {"PGLB_V5_GEO": "2"}]
+# 32: one column batch per task; 64: every row longer than 64 slots cut; 160: 20 groups of 8 slots per full task, not
+# a multiple of either ring's 3 or 4 groups; 1024: the snap limit, so the ladder's 1024-slot row stays whole and its
+# 1025-slot row is cut; 2048: the default's largest task
+CHILD_ENVS = [{"PGLB_STREAM_TASK": t} for t in ("64", "2048", "32", "160", "1024")]
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("env", CHILD_ENVS, ids=["%s=%s" % next(iter(e.items())) for e in CHILD_ENVS])
 def test_per_process_switches_in_child(env):
-    """Task size 64 (every row longer than 64 slots cut, partials + fix-up) and 2048, the per-lane LDGSTS ring and
-    both pinned ring geometries: the numeric tests again, in a child process with the switch set."""
+    """Pinned task sizes (rows longer than T cut, partials + fix-up; at T = 64 both queue orders of spmm_v5_kernel): the
+    numeric tests again, in a child process with the switch set."""
     if CHILD:
         pytest.skip("already the child")
-    sel = "copy_exact or (ue_exact and 128-head) or (task_handout and 0-)" if "PGLB_STREAM_TASK" in env else \
-        "copy_exact"
+    sel = "copy_exact or (ue_exact and 128-head) or v5_queue_orders"
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-q", "-x", "-m", "gpu", "-k", sel,
                         "-p", "no:cacheprovider"], env=dict(os.environ, PGLB_EXACT_CHILD="1", **env),
                        stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=1200)
@@ -863,7 +897,7 @@ def _route_calls():
         ti = "float" if dtype == torch.float32 else "__nv_bfloat16"
 
         def pred(a):
-            return a[0] == ti and a[2:5] == [scaled, d128, hot] and tuple(a[5:8]) == grp
+            return a[0] == ti and a[1:4] == [scaled, d128, hot] and tuple(a[4:7]) == grp
         return family("spmm_v5_kernel", pred, "v5 %s D128=%s hot=%s scaled=%s geo=%d" %
                       ("32" if ti == "float" else "16", d128, hot, scaled, geo))
 

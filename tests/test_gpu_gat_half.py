@@ -84,25 +84,23 @@ def _fused_raw(pgl, csr, f2, a_s, a_d, slope, H, Dh):
 @pytest.mark.parametrize("dtype", DTYPES)
 @pytest.mark.parametrize("H,Dh", [(8, 16), (4, 32), (16, 8), (12, 8)])
 @pytest.mark.parametrize("slope", [0.2, 0.0, 1.0])
-def test_forward_is_round16_of_fp32(pgl, graph, monkeypatch, dtype, H, Dh, slope):
+def test_forward_is_round16_of_fp32(pgl, graph, dtype, H, Dh, slope):
     g, _ = graph
     ops = pgl.ops
     csr = g._fwd_csr()
     N = int(g.num_nodes)
     f = _rand((N, H, Dh), 401 + H, dtype)
     a_s, a_d = _rand((N, H), 402), _rand((N, H), 403)
-    for mode in ("0", "2"):   # PGLB_GAT_DYN: static task map and the device-side queue
-        monkeypatch.setenv("PGLB_GAT_DYN", mode)
-        with torch.no_grad():
-            want = ops.gat_fused(csr, f.float(), a_s, a_d, slope)
-            got = ops.gat_fused(csr, f, a_s, a_d, slope, out_dtype=dtype)
-        assert got.dtype == dtype and torch.equal(_bits(got), _bits(want.to(dtype))), mode
-        out32, lse32 = _fused_raw(pgl, csr, f.float().reshape(N, -1), a_s, a_d, slope, H, Dh)
-        out16, lse16 = _fused_raw(pgl, csr, f.reshape(N, -1), a_s, a_d, slope, H, Dh)
-        assert torch.equal(_bits(out16), _bits(out32.to(dtype))), mode
-        assert torch.equal(lse16.view(torch.int32), lse32.view(torch.int32)), mode
-        tr = ops.gat_fused_train(csr, g._bwd_csr, f, a_s, a_d, slope, out_dtype=dtype)
-        assert tr is not None and torch.equal(_bits(tr), _bits(want.to(dtype))), mode
+    with torch.no_grad():
+        want = ops.gat_fused(csr, f.float(), a_s, a_d, slope)
+        got = ops.gat_fused(csr, f, a_s, a_d, slope, out_dtype=dtype)
+    assert got.dtype == dtype and torch.equal(_bits(got), _bits(want.to(dtype)))
+    out32, lse32 = _fused_raw(pgl, csr, f.float().reshape(N, -1), a_s, a_d, slope, H, Dh)
+    out16, lse16 = _fused_raw(pgl, csr, f.reshape(N, -1), a_s, a_d, slope, H, Dh)
+    assert torch.equal(_bits(out16), _bits(out32.to(dtype)))
+    assert torch.equal(lse16.view(torch.int32), lse32.view(torch.int32))
+    tr = ops.gat_fused_train(csr, g._bwd_csr, f, a_s, a_d, slope, out_dtype=dtype)
+    assert tr is not None and torch.equal(_bits(tr), _bits(want.to(dtype)))
     # the default result dtype is unchanged: torch promotion (bf16 features with fp32 attention give fp32)
     with torch.no_grad():
         assert torch.equal(ops.gat_fused(csr, f, a_s, a_d, slope), want)

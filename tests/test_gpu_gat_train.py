@@ -1,8 +1,6 @@
 """Fused GAT under autograd (pglb_gat_fused_train_csr_f32 + pglb_gat_bwd_edge_f32) and the device-side task queue of
-the persistent kernels (PGLB_V5_DYN / PGLB_GAT_DYN): forward against the oracle restatement of
-pgl/nn/conv.py:308-346, every gradient against plain torch fp32 autograd of the same formula."""
-import os
-
+the persistent kernels: forward against the oracle restatement of pgl/nn/conv.py:308-346, every gradient against plain
+torch fp32 autograd of the same formula."""
 import numpy as np
 import pytest
 import torch
@@ -44,23 +42,6 @@ def torch_gat(f, a_s, a_d, src, dst, n, slope):
     s = torch.zeros((n, H), device=z.device).index_add(0, dst, p)
     al = p / s[dst]
     return torch.zeros_like(f).index_add(0, dst, f[src] * al.unsqueeze(-1)), al
-
-
-class env(object):
-    def __init__(self, **kw):
-        self.kw = kw
-
-    def __enter__(self):
-        self.old = {k: os.environ.get(k) for k in self.kw}
-        for k, v in self.kw.items():
-            os.environ[k] = str(v)
-
-    def __exit__(self, *a):
-        for k, v in self.old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
 
 
 @pytest.mark.parametrize("H,Dh", [(8, 16), (4, 32), (16, 8), (12, 8)])
@@ -196,11 +177,12 @@ def test_gat_fused_train_unsupported_shapes_fall_back(pgl):
 
 
 # ---------------------------------------------------------------- device-side task queue
-@pytest.mark.parametrize("mode", [1, 2])
-def test_dynamic_task_queue_is_bit_identical(pgl, mode):
-    """PGLB_V5_DYN / PGLB_GAT_DYN = 1 (ascending queue), 2 (descending): which warp runs a task does not enter the
-    arithmetic, so the copy-sum result is bit-identical to the static map and the GAT result too (hub rows cut into
-    task partials included: the merge kernels add them in task order)."""
+@pytest.mark.parametrize("order", [1, 2])
+def test_dynamic_task_queue_is_bit_identical(pgl, order):
+    """Which warp runs a task does not enter the arithmetic, and every launch's plan kernel re-arms the queue head that
+    the copy-sum and GAT kernels share through the workspace: repeat launches give the same bits, copy-sum and GAT
+    alike (hub rows cut into task partials included: the merge kernels add them in task order).  order 1: each call
+    repeated back to back; 2: the calls interleaved."""
     n, e, d = 6000, 200000, 128
     edges = O.chung_lu_edges(n, e, exponent=0.9, seed=341)
     g = make_graph(pgl, edges, n)
@@ -209,40 +191,35 @@ def test_dynamic_task_queue_is_bit_identical(pgl, mode):
     norm = torch.rand(n, device="cuda", generator=gen) + 0.5
     a_s = torch.randn(n, 8, device="cuda", generator=gen)
     a_d = torch.randn(n, 8, device="cuda", generator=gen)
+    calls = [lambda: g._send_u_recv(x, "sum", None),
+             lambda: g._send_u_recv(x, "sum", None, scale_src=norm, scale_dst=norm),
+             lambda: g._send_u_recv(x[:, :100].contiguous(), "mean", None),
+             lambda: pgl.ops.gat_fused(g._fwd_csr(), x.reshape(n, 8, 16), a_s, a_d, 0.2)]
     with torch.no_grad():
-        with env(PGLB_V5_DYN=0, PGLB_GAT_DYN=0):
-            base_sum = g._send_u_recv(x, "sum", None)
-            base_gcn = g._send_u_recv(x, "sum", None, scale_src=norm, scale_dst=norm)
-            base_mean = g._send_u_recv(x[:, :100].contiguous(), "mean", None)
-            base_gat = pgl.ops.gat_fused(g._fwd_csr(), x.reshape(n, 8, 16), a_s, a_d, 0.2)
-        with env(PGLB_V5_DYN=mode, PGLB_GAT_DYN=mode):
-            for _ in range(3):   # the queue head is re-armed by every launch's plan kernel
-                assert torch.equal(g._send_u_recv(x, "sum", None), base_sum)
-                assert torch.equal(g._send_u_recv(x, "sum", None, scale_src=norm, scale_dst=norm), base_gcn)
-                assert torch.equal(g._send_u_recv(x[:, :100].contiguous(), "mean", None), base_mean)
-                assert torch.equal(pgl.ops.gat_fused(g._fwd_csr(), x.reshape(n, 8, 16), a_s, a_d, 0.2), base_gat)
+        base = [c() for c in calls]
+        seq = [i for i in range(len(calls)) for _ in range(3)] if order == 1 else list(range(len(calls))) * 3
+        for i in seq:
+            assert torch.equal(calls[i](), base[i]), i
+    base_sum = base[0]
     want = O.send_u_recv(x.cpu().numpy(), edges[:, 0], edges[:, 1], "sum")
     assert rel_err(base_sum.cpu().numpy(), want) <= RTOL
 
 
 def test_dynamic_task_queue_large_graph(pgl):
-    """More tasks than resident warps (the persistent grid is 2 CTAs per SM): 3M edges at T = 32 * k."""
+    """More tasks than resident warps (the persistent grid is 2 CTAs per SM): 3M edges at T = 32 * k, repeat launches
+    bit-identical."""
     n, e, d = 200000, 3000000, 128
     edges = O.chung_lu_edges(n, e, exponent=0.8, seed=351)
     g = make_graph(pgl, edges, n)
     x = torch.randn(n, d, device="cuda")
     with torch.no_grad():
-        with env(PGLB_V5_DYN=0):
-            base = g._send_u_recv(x, "sum", None)
-        for mode in (1, 2):
-            with env(PGLB_V5_DYN=mode):
-                assert torch.equal(g._send_u_recv(x, "sum", None), base)
+        base = g._send_u_recv(x, "sum", None)
+        for _ in range(2):
+            assert torch.equal(g._send_u_recv(x, "sum", None), base)
         a = torch.randn(n, 8, device="cuda")
-        with env(PGLB_GAT_DYN=0):
-            gb = pgl.ops.gat_fused(g._fwd_csr(), x.reshape(n, 8, 16), a, a, 0.2)
-        for mode in (1, 2):
-            with env(PGLB_GAT_DYN=mode):
-                assert torch.equal(pgl.ops.gat_fused(g._fwd_csr(), x.reshape(n, 8, 16), a, a, 0.2), gb)
+        gb = pgl.ops.gat_fused(g._fwd_csr(), x.reshape(n, 8, 16), a, a, 0.2)
+        for _ in range(2):
+            assert torch.equal(pgl.ops.gat_fused(g._fwd_csr(), x.reshape(n, 8, 16), a, a, 0.2), gb)
 
 
 # ---------------------------------------------------------------- attention projections

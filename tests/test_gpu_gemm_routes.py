@@ -1,5 +1,5 @@
-"""Every tensor-core GEMM route -- the dense transform (pglb_linear_tf32x3_f32: linear_wgmma_kernel and the four
-linear_tf32x3_kernel<N, WARPS>) and RGCNConv's forward, grad x and grad W (rgcn_agg_kernel<NP>,
+"""Every tensor-core GEMM route -- the dense transform (pglb_linear_tf32x3_f32: linear_wgmma_kernel and the two
+linear_tf32x3_kernel<N>) and RGCNConv's forward, grad x and grad W (rgcn_agg_kernel<NP>,
 rgcn_wgrad_kernel<DP, NP>, rgcn_wsum_kernel) -- bit for bit against an exact float64 reference.
 
 What each kernel claims to compute.  Every operand v is split into tf32 halves and three products are accumulated in
@@ -34,15 +34,11 @@ scaled by powers of two over +-30 so that small rows are checked at their own sc
 permuting x's rows permutes the output's rows, and scaling a row by 2^s scales its output row by 2^s.
 
 The C entries are also called through ctypes with strided x (NaN in the padding) and an output view inside a wider,
-sentinel-filled buffer (ldo > N, rows after M): every sentinel must survive.  PGLB_LINEAR_WGMMA is read once per
-process, so K = N = 128 on the mma.sync kernel runs in a child process; `test_route_coverage` records the kernels each
-case launches (torch.profiler) and asserts that every instantiation was reached and that each case ran where it
-claims."""
+sentinel-filled buffer (ldo > N, rows after M): every sentinel must survive.  `test_route_coverage` records the
+kernels each case launches (torch.profiler) and asserts that every instantiation was reached and that each case ran
+where it claims."""
 import ctypes
-import os
 import re
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -51,7 +47,6 @@ import torch
 from oracle import oracle_conv as OC
 from test_gpu_exact_routes import _kernels_of
 
-CHILD = os.environ.get("PGLB_GEMM_CHILD") == "1"
 NB = 1021                       # distinct x rows of a dense regime case; longer cases repeat them with period NB
 M_LADDER = ("1", "2", "15", "16", "17", "63", "64", "65", "127", "128", "129", "193", "wg-1", "wg", "wg+1",
             "mma-1", "mma+1", "laps")
@@ -611,10 +606,17 @@ def linear(x, w, b=None, act=None):
     return ops._linear_tc_raw(x, w, b, act)
 
 
-def check_dense(M, K, N, regime, x_trunc, with_bias, act, label):
+def _window(x, pad):
+    """x on the device, read in place from a buffer with `pad` NaN columns after each row (ldx = K + pad)."""
+    buf = torch.full((x.shape[0], x.shape[1] + pad), float("nan"), device="cuda")
+    buf[:, :x.shape[1]] = _cuda(x)
+    return buf[:, :x.shape[1]]
+
+
+def check_dense(M, K, N, regime, x_trunc, with_bias, act, label, pad=0):
     x, w, b, ref = dense_ref(regime, K, N, x_trunc, with_bias, act)
     idx = np.arange(M) % x.shape[0]
-    out = linear(_cuda(x[idx]), _cuda(w), _cuda(b) if b is not None else None, act)
+    out = linear(_window(x[idx], pad), _cuda(w), _cuda(b) if b is not None else None, act)
     torch.cuda.synchronize()
     assert_exact(out, ref[idx], "%s M=%d K=%d N=%d regime %s bias=%s act=%s" % (label, M, K, N, regime, with_bias,
                                                                               act), tile=128 if x_trunc else 64)
@@ -630,9 +632,7 @@ VARIANTS = [("D", False, None), ("D", True, "relu"), ("L", False, None), ("L", T
 @pytest.mark.gpu
 @pytest.mark.parametrize("mlabel", M_LADDER)
 def test_linear_exact_m_ladder(mlabel):
-    """Every M of the ladder on wgmma (K = N = 128) and on the mma.sync kernel (8 warps), both regimes."""
-    if CHILD:
-        pytest.skip("parent only")
+    """Every M of the ladder on wgmma (K = N = 128) and on the mma.sync kernel, both regimes."""
     M = m_of(mlabel)
     for K, N, tr, label in ((128, 128, True, "wgmma"), (128, 64, False, "mma.sync"), (60, 128, False, "mma.sync")):
         for regime, wb, act in VARIANTS:
@@ -640,52 +640,22 @@ def test_linear_exact_m_ladder(mlabel):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("warps,N", [("8", 64), ("8", 128), ("16", 64), ("16", 128)])
-def test_linear_exact_k_ladder(monkeypatch, warps, N):
-    """Every multiple of 4 in [4, 128] at 8 warps, a subset at 16 (PGLB_LINEAR_WARPS is read per call); K = N = 128
-    runs on wgmma here, and on the mma.sync kernel in the child."""
-    if CHILD:
-        pytest.skip("parent only")
-    monkeypatch.setenv("PGLB_LINEAR_WARPS", warps)
-    ks = range(4, 129, 4) if warps == "8" else (4, 8, 12, 28, 36, 64, 68, 100, 124, 128)
+@pytest.mark.parametrize("pad,N", [("8", 64), ("8", 128), ("16", 64), ("16", 128)])
+def test_linear_exact_k_ladder(pad, N):
+    """Every multiple of 4 in [4, 128] with x read in place at ldx = K + 8, a subset at ldx = K + 16 (NaN in the
+    padding); K = N = 128 runs on wgmma (its TMA box strides over the padding), every other K on the mma.sync kernel."""
+    ks = range(4, 129, 4) if pad == "8" else (4, 8, 12, 28, 36, 64, 68, 100, 124, 128)
     for K in ks:
-        if K == 128 and N == 128:
-            continue
+        tr = K == 128 and N == 128
         for regime, wb, act in VARIANTS[:4]:
-            check_dense(193, K, N, regime, False, wb, act, "mma.sync warps=%s" % warps)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("warps", ["8", "16"])
-def test_linear_exact_mma_sync_k128(monkeypatch, warps):
-    """K = N = 128 on linear_tf32x3_kernel<128, 8 | 16>: runs only in the child with PGLB_LINEAR_WGMMA=0."""
-    if not CHILD:
-        pytest.skip("runs in the child (test_linear_mma_sync_k128_in_child)")
-    monkeypatch.setenv("PGLB_LINEAR_WARPS", warps)
-    for mlabel in ("1", "17", "64", "65", "193", "mma-1", "mma+1", "laps"):
-        for regime, wb, act in VARIANTS:
-            check_dense(m_of(mlabel), 128, 128, regime, False, wb, act, "mma.sync k128 warps=%s" % warps)
-    _check_bounds_call(128, 128, 5000, "mma.sync k128 warps=%s" % warps)
-
-
-@pytest.mark.gpu
-def test_linear_mma_sync_k128_in_child():
-    """PGLB_LINEAR_WGMMA=0 (read once per process): the K = N = 128 exact cases and their route coverage in a child."""
-    if CHILD:
-        pytest.skip("already the child")
-    sel = "linear_exact_mma_sync_k128 or route_coverage"
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-q", "-x", "-m", "gpu", "-k", sel,
-                        "-p", "no:cacheprovider"], env=dict(os.environ, PGLB_GEMM_CHILD="1", PGLB_LINEAR_WGMMA="0"),
-                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=1200)
-    assert r.returncode == 0, r.stdout[-4000:]
-    assert " passed" in r.stdout and " failed" not in r.stdout, r.stdout[-2000:]
+            check_dense(193, K, N, regime, tr, wb, act, "wgmma" if tr else "mma.sync", pad=int(pad))
 
 
 SENT = np.array([0x7fc0beef], np.uint32).view(np.float32)[0]     # a NaN with a payload: only a write changes it
 
 
-def _check_bounds_call(K, N, M, what, act=1):
-    """The C entry with x strided (ldx = K + 12, NaN in the padding and in the rows after M) and out a view at
+def _check_bounds_call(K, N, M, what, act=1, xpad=12):
+    """The C entry with x strided (ldx = K + xpad, NaN in the padding and in the rows after M) and out a view at
     (1, 2) inside a sentinel-filled buffer with ldo = N + 6 and 70 rows after M: the sentinels survive and the
     in-bounds values equal the contiguous call's bit for bit."""
     from pgl_b200 import ops
@@ -693,7 +663,7 @@ def _check_bounds_call(K, N, M, what, act=1):
     x = rng.standard_normal((M, K)).astype(np.float32)
     w = rng.standard_normal((K, N)).astype(np.float32)
     b = rng.standard_normal(N).astype(np.float32)
-    ldx, ldo = K + 12, N + 6
+    ldx, ldo = K + xpad, N + 6
     xb = torch.full((M + 3, ldx), float("nan"), device="cuda")
     xb[:M, :K] = _cuda(x)
     ob = torch.empty((M + 71, ldo), device="cuda")
@@ -722,15 +692,12 @@ def _check_bounds_call(K, N, M, what, act=1):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("warps", ["8", "16"])
-def test_linear_output_bounds(monkeypatch, warps):
-    if CHILD:
-        pytest.skip("parent only")
-    monkeypatch.setenv("PGLB_LINEAR_WARPS", warps)
+@pytest.mark.parametrize("pad", ["8", "16"])
+def test_linear_output_bounds(pad):
     sm = _sm()
     for K, N, M in ((128, 128, sm * 128 + 77), (128, 128, 100), (128, 64, sm * 64 + 3), (100, 128, 1000),
                     (36, 64, 77), (4, 128, 5)):
-        _check_bounds_call(K, N, M, "K=%d N=%d M=%d warps=%s" % (K, N, M, warps), act=M % 2)
+        _check_bounds_call(K, N, M, "K=%d N=%d M=%d ldx=K+%s" % (K, N, M, pad), act=M % 2, xpad=int(pad))
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -741,14 +708,11 @@ LIN_RANDOM = [(128, 128, "8"), (128, 64, "8"), (100, 128, "16"), (128, 64, "16")
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("K,N,warps", LIN_RANDOM)
-def test_linear_random_identities_and_bounds(monkeypatch, K, N, warps):
+@pytest.mark.parametrize("K,N,pad", LIN_RANDOM)
+def test_linear_random_identities_and_bounds(K, N, pad):
     """Rows permuted -> output rows permuted bit for bit; a row times 2^s -> its output row times 2^s bit for bit
-    (no bias, s in [-30, 30]); and every element of a call on rows scaled by 2^[-30, 30], with bias and ReLU,
-    within gemm_bound of the float64 product."""
-    if CHILD:
-        pytest.skip("parent only")
-    monkeypatch.setenv("PGLB_LINEAR_WARPS", warps)
+    (no bias, s in [-30, 30]); and every element of a call on rows scaled by 2^[-30, 30], with bias and ReLU, read in
+    place at ldx = K + pad, within gemm_bound of the float64 product."""
     x_trunc = K == 128 and N == 128
     M = _sm() * 128 * 2 + 77
     rng = np.random.default_rng(K * N)
@@ -762,11 +726,11 @@ def test_linear_random_identities_and_bounds(monkeypatch, K, N, warps):
     s = rng.integers(-30, 31, (M, 1))
     xs = (x * np.exp2(s)).astype(np.float32)
     assert_exact(linear(_cuda(xs), wd), base.double().cpu().numpy() * np.exp2(s), "row scaling K=%d N=%d" % (K, N))
-    got = linear(_cuda(xs), wd, _cuda(b), "relu")
+    got = linear(_window(xs, int(pad)), wd, _cuda(b), "relu")
     x64, w64 = xs.astype(np.float64), w.astype(np.float64)
     pre = x64 @ w64 + b
     bound = gemm_bound(np.abs(x64) @ np.abs(w64), (K + 7) & ~7, x_trunc, np.abs(b)[None, :])
-    assert_within(got, np.maximum(pre, 0.0), bound, "per-element bound K=%d N=%d warps=%s" % (K, N, warps))
+    assert_within(got, np.maximum(pre, 0.0), bound, "per-element bound K=%d N=%d" % (K, N))
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -840,8 +804,6 @@ def rgcn_bounds_call(fwd, x, w3, want, what):
 def test_rgcn_exact(D, O, R):
     """Forward, grad x and grad W bit for bit on the regime graph (integer W, hub runs up to 8192 slots), the forward
     once more through the C entry with ldo > N, and grad W of the relation without runs exactly 0."""
-    if CHILD:
-        pytest.skip("parent only")
     el, pool, m, fwd, bwd = rgcn_setup(R, False)
     x, w3, g = rgcn_operands(RGCN_N, R, D, O, pool, D * 1000 + O)
     want_o, want_gx, want_gw, _ = rgcn_refs(m, x, w3, g)
@@ -860,8 +822,6 @@ def test_rgcn_exact(D, O, R):
 def test_rgcn_exact_lo_weights(D, O, R):
     """Forward and grad x bit for bit with a lo-bearing W (a partial permutation of s (h + l 2^-14) values) on a
     graph of short runs, few relations per row and at most 3 out-edges per node; grad W with it."""
-    if CHILD:
-        pytest.skip("parent only")
     el, pool, m, fwd, bwd = rgcn_setup(R, True)
     x, w3, g = rgcn_operands(RGCN_N, R, D, O, pool, D * 1000 + O + 1, lo_w=True)
     want_o, want_gx, want_gw, _ = rgcn_refs(m, x, w3, g)
@@ -878,8 +838,6 @@ def test_rgcn_random_bounds_and_permutation(D, O, R):
     """Random x, W, g on the regime graph: every element of the forward, grad x and grad W within gemm_bound of the
     float64 product of the emulated A tiles; and relabelling the nodes (eid order inside runs kept) permutes the
     forward's rows bit for bit."""
-    if CHILD:
-        pytest.skip("parent only")
     from pgl_b200 import ops
     from pgl_b200.heter_graph import typed_csr
     el, pool, m, fwd, bwd = rgcn_setup(R, False)
@@ -914,8 +872,7 @@ def test_rgcn_random_bounds_and_permutation(D, O, R):
 
 ROUTES = {"linear_wgmma": r"linear_wgmma_kernel"}
 for _n in (64, 128):
-    for _w in (8, 16):
-        ROUTES["linear_tf32x3<%d, %d>" % (_n, _w)] = r"linear_tf32x3_kernel<%d, %d>" % (_n, _w)
+    ROUTES["linear_tf32x3<%d>" % _n] = r"linear_tf32x3_kernel<%d>" % _n
 for _np in (32, 64, 128):
     ROUTES["rgcn_agg<%d>" % _np] = r"rgcn_agg_kernel<%d>" % _np
     for _dp in (64, 128):
@@ -932,22 +889,12 @@ def _route_calls():
     """(label, call, [routes the call must reach, and only these among the GEMM kernels])."""
     calls = []
 
-    def lin(K, N, warps):
+    def lin(K, N):
         x, w, b, _ = dense_ref("D", K, N, K == 128 and N == 128, True, "relu")
-
-        def fn():
-            os.environ["PGLB_LINEAR_WARPS"] = warps
-            linear(_cuda(x), _cuda(w), _cuda(b), "relu")
-        return fn
-    if CHILD:
-        for warps in ("8", "16"):
-            calls.append(("K=N=128 warps=%s" % warps, lin(128, 128, warps), ["linear_tf32x3<128, %s>" % warps]))
-        return calls
-    for warps in ("8", "16"):
-        calls.append(("K=N=128 warps=%s" % warps, lin(128, 128, warps), ["linear_wgmma"]))
-        for K, N in ((128, 64), (100, 128), (4, 64)):
-            calls.append(("K=%d N=%d warps=%s" % (K, N, warps), lin(K, N, warps),
-                          ["linear_tf32x3<%d, %s>" % (N, warps)]))
+        return lambda: linear(_cuda(x), _cuda(w), _cuda(b), "relu")
+    calls.append(("K=N=128", lin(128, 128), ["linear_wgmma"]))
+    for K, N in ((128, 64), (100, 128), (4, 64)):
+        calls.append(("K=%d N=%d" % (K, N), lin(K, N), ["linear_tf32x3<%d>" % N]))
     for D, O, R in RGCN_CASES:
         def fn(D=D, O=O, R=R):
             _, pool, _, fwd, bwd = rgcn_setup(R, False)
@@ -960,30 +907,20 @@ def _route_calls():
 
 @pytest.mark.gpu
 def test_route_coverage():
-    """Each case reaches the kernels it claims and no other GEMM kernel; together (with the child's K = N = 128
-    calls) they reach every instantiation."""
+    """Each case reaches the kernels it claims and no other GEMM kernel; together they reach every instantiation."""
     a = torch.ones(1024, device="cuda")
     names, _ = _kernels_of(lambda: a.add_(1))
     if not names:
         pytest.skip("torch.profiler records no CUDA kernels here (probe: a plain torch kernel)")
-    old = os.environ.get("PGLB_LINEAR_WARPS")
     hit, failures = set(), []
-    try:
-        for label, fn, claims in _route_calls():
-            names, _ = _kernels_of(fn)
-            gemm = sorted({mt.group(0) for mt in (_GEMM.search(nm) for nm in names) if mt})
-            reached = {r for r, pat in ROUTES.items() if any(re.search(pat + r"(?![\d])", nm) for nm in gemm)}
-            if reached != set(claims):
-                failures.append("%s: expected %s; launched %s" % (label, sorted(claims), gemm))
-            hit |= reached
-    finally:
-        if old is None:
-            os.environ.pop("PGLB_LINEAR_WARPS", None)
-        else:
-            os.environ["PGLB_LINEAR_WARPS"] = old
+    for label, fn, claims in _route_calls():
+        names, _ = _kernels_of(fn)
+        gemm = sorted({mt.group(0) for mt in (_GEMM.search(nm) for nm in names) if mt})
+        reached = {r for r, pat in ROUTES.items() if any(re.search(pat + r"(?![\d])", nm) for nm in gemm)}
+        if reached != set(claims):
+            failures.append("%s: expected %s; launched %s" % (label, sorted(claims), gemm))
+        hit |= reached
     assert not failures, "\n".join(failures)
-    expect = {"linear_tf32x3<128, 8>", "linear_tf32x3<128, 16>"} if CHILD else \
-        set(ROUTES)
-    missing = sorted(expect - hit)
+    missing = sorted(set(ROUTES) - hit)
     assert not missing, "routes not reached: %s" % missing
-    print("GEMM routes reached%s: %s" % (" (child, PGLB_LINEAR_WGMMA=0)" if CHILD else "", sorted(hit)))
+    print("GEMM routes reached: %s" % sorted(hit))

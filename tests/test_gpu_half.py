@@ -149,21 +149,16 @@ def _agree_across_packings(digests):
 
 
 def test_wide_rows_bit_identical_to_rounded_fp32():
-    """Bulk-copy issue mode (the default), every packing, both geometries, both norms: round16(fp32) bit for bit,
-    and every packing agrees.  The LDGSTS ring (PGLB_STREAM_V5=2) gives the same bits in a child."""
+    """Every packing, both geometries, both norms: round16(fp32) bit for bit, and every packing agrees."""
     bad, mine = _wide_row_report()
     assert bad == []
     assert _agree_across_packings(mine) == {}
-    bad2, ring = _child({"PGLB_STREAM_V5": "2"})
-    assert bad2 == [] and ring == mine
 
 
 def test_wide_rows_bit_identical_with_short_tasks():
     """64-slot tasks cut hub rows into fp32 partials that the 16-bit fix-up kernel adds and rounds once."""
     bad, short = _child({"PGLB_STREAM_TASK": "64"})
     assert bad == [] and _agree_across_packings(short) == {}
-    bad2, ring = _child({"PGLB_STREAM_TASK": "64", "PGLB_STREAM_V5": "2"})
-    assert bad2 == [] and ring == short
 
 
 # 3. the bar for scaled calls on the node-parallel kernel and cut hub rows -------------------------------------------

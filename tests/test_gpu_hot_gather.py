@@ -1,8 +1,8 @@
 """Hot rows of the wide-row aggregation (spmm_v5_kernel with L2 hints, D = 128): a row whose packed id has bit 31 set
-is gathered by per-lane cp.async, every other row by a bulk copy.  The output must be bit for bit what the kernel gives
-with no hints (every row by bulk copy) and what the per-lane LDGSTS ring (PGLB_STREAM_V5=2) gives: for groups that
-are all cold, mixed and all hot, in both ring geometries, with streamed and gathered source norms, for the unscaled sum
-and the mean, with hub rows cut into task partials and with empty rows."""
+is gathered by per-lane cp.async (LDGSTS), every other row by a bulk copy.  The output must be bit for bit what the
+kernel gives with no hints (every row by bulk copy) and with every row hot (every row by per-lane LDGSTS): for groups
+that are all cold, mixed and all hot, in both ring geometries, with streamed and gathered source norms, for the
+unscaled sum and the mean, with hub rows cut into task partials and with empty rows."""
 import hashlib
 import json
 import os
@@ -76,18 +76,13 @@ def _child(env):
 
 @pytest.mark.gpu
 def test_hot_rows_bit_identical_to_bulk_and_ldgsts_ring():
-    """Every packing agrees with the no-hint (all bulk copy) output, and the per-lane LDGSTS ring, read once per
-    process, gives the same bits in a child."""
-    mine = _digests()
-    assert _mismatches(mine) == {}
-    ring = _child({"PGLB_STREAM_V5": "2"})
-    assert ring == mine
+    """Every packing agrees with the no-hint (all bulk copy) output, the every-row-hot packing (all per-lane LDGSTS)
+    included."""
+    assert _mismatches(_digests()) == {}
 
 
 @pytest.mark.gpu
 def test_hot_rows_bit_identical_with_short_tasks():
     """Tasks of 64 slots cut every hub row into partials added by the fix-up kernel: the hybrid gather agrees with
-    the no-hint output and with the LDGSTS ring at the same task size."""
-    short = _child({"PGLB_STREAM_TASK": "64"})
-    assert _mismatches(short) == {}
-    assert _child({"PGLB_STREAM_TASK": "64", "PGLB_STREAM_V5": "2"}) == short
+    the no-hint and the every-row-hot outputs at that task size."""
+    assert _mismatches(_child({"PGLB_STREAM_TASK": "64"})) == {}

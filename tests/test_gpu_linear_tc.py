@@ -21,14 +21,15 @@ def rel_err(a, b):
     return float((a - b).abs().max() / b.abs().max().clamp(min=1e-12))
 
 
-@pytest.mark.parametrize("warps", ["8", "16"])
+@pytest.mark.parametrize("pad", ["8", "16"])   # x read in place from a buffer with `pad` NaN columns after each row
 @pytest.mark.parametrize("M,K,N", [(5000, 128, 128), (4097, 100, 128), (10000, 64, 64), (6401, 8, 64),
                                    (64, 128, 128), (1, 4, 128), (70001, 128, 64),
                                    (70001, 128, 128)])
-def test_linear_tc_matches_fp64(pgl, monkeypatch, M, K, N, warps):
-    monkeypatch.setenv("PGLB_LINEAR_WARPS", warps)  # both CTA shapes of the kernel
+def test_linear_tc_matches_fp64(pgl, M, K, N, pad):
     gen = torch.Generator(device="cuda").manual_seed(M + K + N)
-    x = torch.randn(M, K, device="cuda", generator=gen) * 3
+    buf = torch.full((M, K + int(pad)), float("nan"), device="cuda")
+    x = buf[:, :K]
+    x.copy_(torch.randn(M, K, device="cuda", generator=gen) * 3)
     w = torch.randn(K, N, device="cuda", generator=gen)
     b = torch.randn(N, device="cuda", generator=gen)
     ref = x.double() @ w.double()

@@ -1,11 +1,8 @@
 """Per-slot source norms of the wide-row aggregation (spmm_v5_kernel): streaming scale_src[cols[j]] per CSR slot must
-give bit for bit what gathering scale_src per edge gives, in both copy mechanisms (PGLB_STREAM_V5 = 1 and 2), both
-ring geometries, D = 128 (with and without L2 hints) and D < 128, with hub rows cut into task partials and with empty
-rows.  Also the caching rule of EdgeIndex.slot_scale and the argument check of the C entry point."""
+give bit for bit what gathering scale_src per edge gives, in both ring geometries, D = 128 (no hints, some rows hot,
+every row hot) and D < 128, with hub rows cut into task partials and with empty rows.  Also the caching rule of EdgeIndex.slot_scale
+and the argument check of the C entry point."""
 import ctypes
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -13,8 +10,6 @@ import torch
 
 from oracle import oracle as O
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 EMPTY = 100  # trailing nodes without any edge: empty rows and never-gathered sources
 
 
@@ -26,8 +21,10 @@ def _graph(pgl, n, e, seed):
     return g, edges
 
 
-def _mismatches():
-    """Every case the v5 kernel takes, streamed vs gathered norms; returns the cases that differ."""
+def _mismatches(all_hot=False):
+    """Every case the v5 kernel takes, streamed vs gathered norms; returns the cases that differ.  all_hot: at D = 128
+    only, bit 31 on every id, so every row comes by per-lane cp.async (LDGSTS) and the gathered norms share its
+    commit groups."""
     import pgl_b200 as pgl
     import pgl_b200.nn.functional as GF
     from pgl_b200 import ops
@@ -39,10 +36,11 @@ def _mismatches():
         fwd = g._fwd_csr()
         norm = GF.degree_norm(g).reshape(-1)
         assert fwd["slot_scale"](norm) is None and fwd["slot_scale"](norm) is not None
-        for D in (128, 96):
+        for D in ((128,) if all_hot else (128, 96)):
             x = torch.randn(N, D, device="cuda", generator=torch.Generator("cuda").manual_seed(D))
-            for budget in (0, 1 << 20):  # no hints / bit 31 marks the 2048 heaviest rows (D = 128 only)
-                pk = tuple(ops.pack_cols(fwd["cols"], N, 4 * D, budget_bytes=budget))
+            for budget in ((None,) if all_hot else (0, 1 << 20)):  # no hints / the 2048 heaviest rows (D = 128 only)
+                pk = (fwd["cols"].to(torch.int32) | -(1 << 31), True) if all_hot else \
+                    tuple(ops.pack_cols(fwd["cols"], N, 4 * D, budget_bytes=budget))
                 outs = [ops._spmm_raw(fwd["indptr"], fwd["cols"], x, N, "sum", scale_src=norm, scale_dst=norm,
                                       max_degree=fwd["max_degree"], packed=p)
                         for p in (pk, ops.PackedCols(pk, fwd["slot_scale"]))]
@@ -58,12 +56,7 @@ def test_streamed_norms_bit_identical_to_gathered():
 
 @pytest.mark.gpu
 def test_streamed_norms_bit_identical_ldgsts_ring():
-    """PGLB_STREAM_V5=2 (per-lane cp.async ring) is read once per process: run the same cases in a child."""
-    env = dict(os.environ, PGLB_STREAM_V5="2")
-    code = ("import sys; sys.path[:0] = [%r, %r]; import test_gpu_slot_scale as t; bad = t._mismatches(); "
-            "print(bad); sys.exit(1 if bad else 0)" % (ROOT, HERE))
-    r = subprocess.run([sys.executable, "-s", "-c", code], env=env, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-4000:]
+    assert _mismatches(all_hot=True) == []
 
 
 @pytest.mark.gpu
