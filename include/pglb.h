@@ -595,6 +595,61 @@ int pglb_gatv2_bwd_edge_drop_x16(const int64_t *rows, const int64_t *cols, const
                                  uint64_t offset, float *beta_e, float *ds_e, float *grad_attn, void *ws,
                                  size_t ws_bytes, void *stream);
 
+/* FAConv's self-gated aggregation (pgl/nn/conv.py:1306-1339: send_uv(g_src, g_dst, add), tanh, the product with
+ * send_uv(norm, norm, mul), dropout, send_ue_recv(feature, alpha, mul, sum)) in ONE pass, no [E] tensor written:
+ *   t_j = tanh(g_src[u] + g_dst[d]),  w_j = keep_j s ((t_j norm[u]) norm[d]),  out[d,:] = sum_j w_j f[u,:]
+ * over the dst-CSR slots j = (u -> d) of row d (rows without in-edges: out = 0).  tanh is full-precision tanhf.
+ *   - rec [n, 4] float32, 16-byte aligned: the node records (g_src[i], norm[i], g_dst[i], 0) -- one 16-byte bulk copy
+ *     per slot.  f [n, D] with row stride ldf, out [n, D] with row stride ldo, in elements.  ws as
+ *     pglb_spmm_csr_ws(n, num_edges, D).
+ *   - Shapes: D <= 128 in 16-byte rows (D % 4 == 0 float32, D % 8 == 0 16-bit), n < 2^31 - 1: otherwise
+ *     PGLB_EUNSUPPORTED.  f, rec, out not 16-byte aligned, a row stride below D or not a multiple of 16 bytes:
+ *     PGLB_ESHAPE.
+ *   - _x16 (`dtype` bfloat16 / float16 f and out; rec float32): rows are widened exactly and every later operation is
+ *     the float32 kernel's in the same slot order, rounded once on the store: out == round16(pglb_fa_attn_csr_f32 on
+ *     the widened f) bit for bit.  Unknown dtype: PGLB_EINVAL.
+ *   - _drop_ (dropout on the edge weights): attn_drop in (0, 1), seed, offset (a multiple of 4) with the stream of the
+ *     GAT dropout entries above: slot j is kept iff bit 0 of its 4-head keep word is set (pglb_attn_dropout_keep_host
+ *     with H = 4, & 1), and s = (float)(1 / (1 - attn_drop)); without dropout keep_j s = 1.
+ *   - All argument checks precede any CUDA call. */
+int pglb_fa_attn_csr_f32(const int64_t *indptr, const int64_t *cols, const float *f, int64_t ldf, const float *rec,
+                         float *out, int64_t ldo, int64_t n, int64_t num_edges, int64_t D, void *ws, size_t ws_bytes,
+                         void *stream);
+int pglb_fa_attn_csr_x16(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf, const float *rec,
+                         void *out, int64_t ldo, int64_t n, int64_t num_edges, int64_t D, int dtype, void *ws,
+                         size_t ws_bytes, void *stream);
+int pglb_fa_attn_drop_csr_f32(const int64_t *indptr, const int64_t *cols, const float *f, int64_t ldf,
+                              const float *rec, float *out, int64_t ldo, int64_t n, int64_t num_edges, int64_t D,
+                              float attn_drop, uint64_t seed, uint64_t offset, void *ws, size_t ws_bytes, void *stream);
+int pglb_fa_attn_drop_csr_x16(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
+                              const float *rec, void *out, int64_t ldo, int64_t n, int64_t num_edges, int64_t D,
+                              int dtype, float attn_drop, uint64_t seed, uint64_t offset, void *ws, size_t ws_bytes,
+                              void *stream);
+
+/* Per-edge part of that aggregation's backward.  rows / cols / eid as pglb_gat_bwd_edge_f32 (eid nullable: identity);
+ * rec the forward's node records; grad_out = G [n, D] with row stride ldg.  With t and w rebuilt by the forward's
+ * function (w the forward's weight bit for bit):
+ *   beta_e[e] = w,   dz_e[e] = keep s ((norm[u] norm[d]) (1 - t^2)) <G[d,:], f[u,:]>
+ * both [num_edges] float32 in ORIGINAL edge order, no atomics.  The caller finishes the gradients on the existing
+ * kernels: grad f = send_ue_recv(G, beta_e, mul, sum) over the src-keyed CSR, grad g_src / grad g_dst = segment sums of
+ * dz_e over the src- / dst-keyed CSR.  Shapes and alignment as the forward's.
+ *   - _x16: f and grad_out in `dtype`, widened exactly; beta_e and dz_e equal the f32 entry's on the widened inputs.
+ *   - _drop_: the forward's attn_drop, seed, offset. */
+int pglb_fa_bwd_edge_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *f, int64_t ldf,
+                         const float *rec, const float *grad_out, int64_t ldg, int64_t num_edges, int64_t D,
+                         float *beta_e, float *dz_e, void *stream);
+int pglb_fa_bwd_edge_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *f, int64_t ldf,
+                         const float *rec, const void *grad_out, int64_t ldg, int64_t num_edges, int64_t D, int dtype,
+                         float *beta_e, float *dz_e, void *stream);
+int pglb_fa_bwd_edge_drop_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *f,
+                              int64_t ldf, const float *rec, const float *grad_out, int64_t ldg, int64_t num_edges,
+                              int64_t D, float attn_drop, uint64_t seed, uint64_t offset, float *beta_e, float *dz_e,
+                              void *stream);
+int pglb_fa_bwd_edge_drop_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *f,
+                              int64_t ldf, const float *rec, const void *grad_out, int64_t ldg, int64_t num_edges,
+                              int64_t D, int dtype, float attn_drop, uint64_t seed, uint64_t offset, float *beta_e,
+                              float *dz_e, void *stream);
+
 /* The score-gradient aggregation of that backward:
  *   out[r, c] (+)= sum over the slots j of row r of ds[eid[j], h(c)] * attn[c] * lrelu'(f[r, c] + f[cols[j], c])
  * lrelu'(x) = 1 if x > 0 else negative_slope (torch's convention at 0).  On the dst-keyed CSR it is the dst term of

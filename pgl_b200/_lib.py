@@ -185,6 +185,18 @@ _SIGS = {
                                           _i64, c_int, _p, c_size_t, _p]),
     "pglb_gatv2_score_grad_x16": (c_int, [_p, _p, _p, _p, _i64, _p, ctypes.c_float, _p, _p, _i64, _i64, _i64, _i64,
                                           _i64, c_int, c_int, _p, c_size_t, _p]),
+    "pglb_fa_attn_csr_f32": (c_int, [_p, _p, _p, _i64, _p, _p, _i64, _i64, _i64, _i64, _p, c_size_t, _p]),
+    "pglb_fa_attn_csr_x16": (c_int, [_p, _p, _p, _i64, _p, _p, _i64, _i64, _i64, _i64, c_int, _p, c_size_t, _p]),
+    "pglb_fa_attn_drop_csr_f32": (c_int, [_p, _p, _p, _i64, _p, _p, _i64, _i64, _i64, _i64, ctypes.c_float, _u64,
+                                          _u64, _p, c_size_t, _p]),
+    "pglb_fa_attn_drop_csr_x16": (c_int, [_p, _p, _p, _i64, _p, _p, _i64, _i64, _i64, _i64, c_int, ctypes.c_float,
+                                          _u64, _u64, _p, c_size_t, _p]),
+    "pglb_fa_bwd_edge_f32": (c_int, [_p, _p, _p, _p, _i64, _p, _p, _i64, _i64, _i64, _p, _p, _p]),
+    "pglb_fa_bwd_edge_x16": (c_int, [_p, _p, _p, _p, _i64, _p, _p, _i64, _i64, _i64, c_int, _p, _p, _p]),
+    "pglb_fa_bwd_edge_drop_f32": (c_int, [_p, _p, _p, _p, _i64, _p, _p, _i64, _i64, _i64, ctypes.c_float, _u64, _u64,
+                                          _p, _p, _p]),
+    "pglb_fa_bwd_edge_drop_x16": (c_int, [_p, _p, _p, _p, _i64, _p, _p, _i64, _i64, _i64, c_int, ctypes.c_float,
+                                          _u64, _u64, _p, _p, _p]),
     "pglb_rgcn_agg_f32": (c_int, [_p, _p, _p, _p, _p, _i64, _p, _i64, _i64, _i64, _p, _i64, _i64, _p]),
     "pglb_rgcn_wgrad_ws": (c_int, [_i64, _i64, _i64, POINTER(c_size_t)]),
     "pglb_rgcn_wgrad_f32": (c_int, [_p, _p, _p, _p, _p, _i64, _i64, _i64, _p, _p, _i64, _p, _i64, _i64, _i64, _p, _p,

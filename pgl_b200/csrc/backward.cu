@@ -403,6 +403,81 @@ __global__ void __launch_bounds__(256) gatv2_bwd_edge_kernel(
     }
 }
 
+// Backward of the single-pass FAConv aggregation (pglb_fa_attn_*), the per-edge part, on gat_bwd_edge_kernel's walk of
+// the dst-CSR slots (rows[] = destination of every slot).  With (t, w) = fa_weight(g_src[src], g_dst[dst], norm[src],
+// norm[dst]) rebuilt -- w the forward's weight bit for bit -- and G = d loss / d out:
+//   beta_e = w,   dz_e = keep s ((norm[src] norm[dst]) (1 - t^2)) <G[dst,:], f[src,:]>     (keep s = 1 without dropout)
+// both [E] fp32 in ORIGINAL edge order: grad f = sum over out-edges of beta G[dst], grad g_src / grad g_dst = segment
+// sums of dz over the src- / dst-CSR.  rec: [n] node records (g_src, norm, g_dst, 0).  A warp owns 32 consecutive
+// slots; each lane loads its own slot's column, edge id, source record (and, DROP, keep word) and the consume loop shuffles
+// them; the D / 4 active lanes hold one float4 of the rows and the dot is summed over the warp.  T: element type of f
+// and G (16-bit rows are widened exactly; everything after that is the float32 kernel's arithmetic).
+template <typename T, bool DROP>
+__global__ void __launch_bounds__(256) fa_bwd_edge_kernel(
+    const int64_t *__restrict__ rows, const int64_t *__restrict__ cols, const int64_t *__restrict__ eid,
+    const T *__restrict__ f, int64_t ldf, const float4 *__restrict__ rec, const T *__restrict__ g, int64_t ldg,
+    int64_t E, int D, float *__restrict__ beta_e, float *__restrict__ dz_e, const AttnDrop drop) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const bool act = lane * 4 < D;
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int64_t base = warp * 32; base < E; base += nwarps * 32) {
+        const int64_t j = base + lane;
+        const bool in = j < E;
+        const long long r_l = in ? ld_stream(rows + j) : 0;
+        const long long c_l = in ? ld_stream(cols + j) : 0;
+        const long long i_l = in ? (eid ? ld_stream(eid + j) : j) : 0;
+        const float4 rs_l = in ? __ldg(rec + c_l) : zero;   // the slot's source record
+        unsigned kw_l = 0;
+        if constexpr (DROP) kw_l = attn_keep_word(drop, (uint64_t)j, 4);
+        const int cnt = (E - base) < 32 ? (int)(E - base) : 32;
+        long long cur = -1;
+        float4 g4 = zero;
+        float gd = 0.f, nd = 0.f;
+        for (int k0 = 0; k0 < cnt; k0 += 4) {
+            float4 fs[4];
+            long long rr[4], ii[4];
+            float gs[4], nu[4];
+            unsigned kk[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const int s = (k0 + u) & 31;
+                const long long cc = __shfl_sync(0xffffffffu, c_l, s);
+                rr[u] = __shfl_sync(0xffffffffu, r_l, s);
+                ii[u] = __shfl_sync(0xffffffffu, i_l, s);
+                gs[u] = __shfl_sync(0xffffffffu, rs_l.x, s);
+                nu[u] = __shfl_sync(0xffffffffu, rs_l.y, s);
+                kk[u] = 1u;
+                if constexpr (DROP) kk[u] = __shfl_sync(0xffffffffu, kw_l, s);
+                fs[u] = zero;
+                if (k0 + u < cnt && act) fs[u] = ldg_row4<T>(f + cc * ldf + lane * 4);
+            }
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                if (k0 + u >= cnt) break;
+                if (rr[u] != cur) {  // warp-uniform
+                    cur = rr[u];
+                    if (act) g4 = ldg_row4<T>(g + cur * ldg + lane * 4);
+                    const float4 rd = __ldg(rec + cur);
+                    gd = rd.z;
+                    nd = rd.y;
+                }
+                const float dot = head_sum_lanes(dot4_lane(g4, fs[u]), 32);
+                const bool keep = kk[u] & 1u;
+                float t;
+                const float w = fa_weight<DROP>(gs[u], gd, nu[u], nd, keep, drop.scale, &t);
+                float dz = ((nu[u] * nd) * (1.0f - t * t)) * dot;
+                if constexpr (DROP) dz = keep ? drop.scale * dz : 0.0f;
+                if (lane == 0) {
+                    beta_e[ii[u]] = w;
+                    dz_e[ii[u]] = dz;
+                }
+            }
+        }
+    }
+}
+
 // grad a[c] = sum over the nb blocks' shares ga_part[b * 128 + c], in a fixed order: block c of the grid, thread t adds
 // b = t, t + 256, ..., then a fixed tree over the threads.
 __global__ void __launch_bounds__(256) gatv2_ga_reduce_kernel(const float *__restrict__ ga_part, int nb,
@@ -907,6 +982,84 @@ extern "C" int pglb_gatv2_bwd_edge_drop_x16(const int64_t *rows, const int64_t *
     return gatv2_bwd_edge_entry<__half>(name, rows, cols, eid, f, ldf, attn, negative_slope, grad_out, ldg, out, ldo,
                                         lse, num_edges, H, head_dim, beta_e, ds_e, grad_attn, ws, ws_bytes, stream_,
                                         &drop);
+}
+
+// The checks and the launch of the FAConv edge-backward entries (include/pglb.h).  T: element type of f and grad_out,
+// rows 16-byte aligned.  drop (nullable): the attention-dropout stream.
+template <typename T>
+static int fa_bwd_edge_entry(const char *name, const int64_t *rows, const int64_t *cols, const int64_t *eid,
+                             const void *f_, int64_t ldf, const float *rec, const void *g_, int64_t ldg,
+                             int64_t num_edges, int64_t D, float *beta_e, float *dz_e, void *stream_,
+                             const AttnDrop *drop) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    const T *f = reinterpret_cast<const T *>(f_), *g = reinterpret_cast<const T *>(g_);
+    constexpr int64_t B = sizeof(T);
+    PGLB_CHECK_ARG(num_edges >= 0 && D > 0, PGLB_EINVAL, "%s: bad size", name);
+    PGLB_CHECK_ARG(D <= 128 && (D * B) % 16 == 0, PGLB_EUNSUPPORTED,
+                   "%s: needs D <= 128 in 16-byte rows (D %% 4 == 0 float32, D %% 8 == 0 16-bit)", name);
+    if (num_edges == 0) return PGLB_OK;
+    PGLB_CHECK_ARG(rows && cols && f && rec && g && beta_e && dz_e, PGLB_EINVAL, "%s: NULL pointer", name);
+    auto a16 = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
+    PGLB_CHECK_ARG(ldf >= D && ldg >= D && (ldf * B) % 16 == 0 && (ldg * B) % 16 == 0 && a16(f) && a16(g) && a16(rec),
+                   PGLB_ESHAPE, "%s: rows must be 16-byte aligned", name);
+    const int grid = grid_of(num_edges, 64);  // a warp per 32 slots, grid-stride
+    const float4 *rec4 = reinterpret_cast<const float4 *>(rec);
+    if (drop)
+        fa_bwd_edge_kernel<T, true><<<grid, 256, 0, stream>>>(rows, cols, eid, f, ldf, rec4, g, ldg, num_edges, (int)D,
+                                                              beta_e, dz_e, *drop);
+    else
+        fa_bwd_edge_kernel<T, false><<<grid, 256, 0, stream>>>(rows, cols, eid, f, ldf, rec4, g, ldg, num_edges,
+                                                               (int)D, beta_e, dz_e, AttnDrop{});
+    PGLB_LAUNCH_CHECK("fa_bwd_edge_kernel");
+    return PGLB_OK;
+}
+
+extern "C" int pglb_fa_bwd_edge_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid, const float *f,
+                                    int64_t ldf, const float *rec, const float *grad_out, int64_t ldg,
+                                    int64_t num_edges, int64_t D, float *beta_e, float *dz_e, void *stream_) {
+    return fa_bwd_edge_entry<float>("pglb_fa_bwd_edge_f32", rows, cols, eid, f, ldf, rec, grad_out, ldg, num_edges, D,
+                                    beta_e, dz_e, stream_, nullptr);
+}
+
+extern "C" int pglb_fa_bwd_edge_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *f,
+                                    int64_t ldf, const float *rec, const void *grad_out, int64_t ldg,
+                                    int64_t num_edges, int64_t D, int dtype, float *beta_e, float *dz_e,
+                                    void *stream_) {
+    const char *name = "pglb_fa_bwd_edge_x16";
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    if (dtype == PGLB_DTYPE_BF16)
+        return fa_bwd_edge_entry<__nv_bfloat16>(name, rows, cols, eid, f, ldf, rec, grad_out, ldg, num_edges, D,
+                                                beta_e, dz_e, stream_, nullptr);
+    return fa_bwd_edge_entry<__half>(name, rows, cols, eid, f, ldf, rec, grad_out, ldg, num_edges, D, beta_e, dz_e,
+                                     stream_, nullptr);
+}
+
+extern "C" int pglb_fa_bwd_edge_drop_f32(const int64_t *rows, const int64_t *cols, const int64_t *eid,
+                                         const float *f, int64_t ldf, const float *rec, const float *grad_out,
+                                         int64_t ldg, int64_t num_edges, int64_t D, float attn_drop, uint64_t seed,
+                                         uint64_t offset, float *beta_e, float *dz_e, void *stream_) {
+    const char *name = "pglb_fa_bwd_edge_drop_f32";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    return fa_bwd_edge_entry<float>(name, rows, cols, eid, f, ldf, rec, grad_out, ldg, num_edges, D, beta_e, dz_e,
+                                    stream_, &drop);
+}
+
+extern "C" int pglb_fa_bwd_edge_drop_x16(const int64_t *rows, const int64_t *cols, const int64_t *eid, const void *f,
+                                         int64_t ldf, const float *rec, const void *grad_out, int64_t ldg,
+                                         int64_t num_edges, int64_t D, int dtype, float attn_drop, uint64_t seed,
+                                         uint64_t offset, float *beta_e, float *dz_e, void *stream_) {
+    const char *name = "pglb_fa_bwd_edge_drop_x16";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    if (dtype == PGLB_DTYPE_BF16)
+        return fa_bwd_edge_entry<__nv_bfloat16>(name, rows, cols, eid, f, ldf, rec, grad_out, ldg, num_edges, D,
+                                                beta_e, dz_e, stream_, &drop);
+    return fa_bwd_edge_entry<__half>(name, rows, cols, eid, f, ldf, rec, grad_out, ldg, num_edges, D, beta_e, dz_e,
+                                     stream_, &drop);
 }
 
 // The keep words of dst-CSR slots slot0 .. slot0 + n_slots - 1 on the host (include/pglb.h): the same attn_keep_word

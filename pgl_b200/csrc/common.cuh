@@ -169,6 +169,19 @@ __device__ __forceinline__ float gatv2_lane(const float4 &a, const float4 &fs, c
                      fmaf(a.y, lrelu_of(fs.y + fd.y, slope), a.x * lrelu_of(fs.x + fd.x, slope))));
 }
 
+// The FAConv edge weight (spmm_gat5_kernel<kScoreFA>, fa_bwd_edge_kernel): t = tanh(gs + gd) in full precision
+// (tanhf, not tanh.approx), w = (t * nu) * nd -- the reference's h * src_norm * dst_norm -- and, with dropout (DROP),
+// w = keep ? s * w : 0.  The forward and the edge backward call this one function, so the backward's beta is the forward's weight
+// bit for bit; *t receives t for the backward's (1 - t^2).
+template <bool DROP>
+__host__ __device__ __forceinline__ float fa_weight(float gs, float gd, float nu, float nd, bool keep, float s,
+                                                    float *t) {
+    *t = tanhf(gs + gd);
+    const float w = (*t * nu) * nd;
+    if constexpr (DROP) return keep ? s * w : 0.0f;
+    else return w;
+}
+
 // ---- attention dropout of the fused GAT training path (the *_drop_* entries) ----------------------------------------
 // The keep decision of dst-CSR slot j (absolute slot index) and head h, for drop probability p:
 //   draw = Philox4x32-10(counter = (j lo32, j hi32, h / 4, offset / 4), key = (seed lo32, seed hi32)) word h % 4

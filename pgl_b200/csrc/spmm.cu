@@ -504,6 +504,14 @@ template <typename T>
 bool gatv2_attn_takes(int64_t D, int64_t head_dim, float slope, const void *f, int64_t ldf, const float *attn,
                       int64_t n_src);
 
+// the fused FAConv aggregation over f / out of element type T, and whether it takes a call
+template <typename T>
+int fa_attn_run(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf, const float *rec, void *out,
+                int64_t ldo, int64_t n, int64_t E, int64_t D, const AttnDrop *drop, void *ws, size_t ws_bytes,
+                cudaStream_t stream);
+template <typename T>
+bool fa_attn_takes(int64_t D, const void *f, int64_t ldf, const float *rec, int64_t n);
+
 // spmm_v5_kernel over rows of element type T (float, __nv_bfloat16 or __half): whether it takes a call, and the run
 template <typename T>
 bool v5_eligible(const int64_t *cols, const uint32_t *cols32, const void *x, int64_t ldx, const void *out, int64_t ldo,
@@ -1345,6 +1353,79 @@ extern "C" int pglb_gatv2_attn_drop_csr_x16(const int64_t *indptr, const int64_t
                                    head_dim, ws, ws_bytes, stream_, &drop);
     };
     return dtype == PGLB_DTYPE_BF16 ? run((__nv_bfloat16 *)nullptr) : run((__half *)nullptr);
+}
+
+// The argument checks and the launch of the FAConv aggregation entries (include/pglb.h).  T: element type of f and
+// out.  Every check precedes any CUDA call.  drop (nullable): the attention-dropout stream.
+template <typename T>
+static int fa_attn_entry(const char *name, const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
+                         const float *rec, void *out, int64_t ldo, int64_t n, int64_t num_edges, int64_t D, void *ws,
+                         size_t ws_bytes, void *stream_, const AttnDrop *drop) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    constexpr int64_t B = sizeof(T);
+    PGLB_CHECK_ARG(n >= 0 && num_edges >= 0 && D > 0, PGLB_EINVAL, "%s: bad size", name);
+    PGLB_CHECK_ARG(D <= 128 && (D * B) % 16 == 0 && num_edges < 0x7fffffffLL && n < 0x7fffffffLL, PGLB_EUNSUPPORTED,
+                   "%s: needs D <= 128 in 16-byte rows (D %% 4 == 0 float32, D %% 8 == 0 16-bit)", name);
+    if (n == 0) return PGLB_OK;
+    PGLB_CHECK_ARG(indptr && out, PGLB_EINVAL, "%s: NULL pointer", name);
+    PGLB_CHECK_ARG(num_edges == 0 || (cols && f && rec), PGLB_EINVAL, "%s: NULL pointer", name);
+    PGLB_CHECK_ARG(ldf >= D && ldo >= D && (ldo * B) % 16 == 0 && aligned16(out) &&
+                       (num_edges == 0 || fa_attn_takes<T>(D, f, ldf, rec, n)),
+                   PGLB_ESHAPE, "%s: rows must be 16-byte aligned", name);
+    if (num_edges == 0) {
+        PGLB_CUDA(cudaMemset2DAsync(out, B * ldo, 0, B * D, n, stream));
+        return PGLB_OK;
+    }
+    PGLB_CHECK_ARG(ws && (reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
+                   "%s: workspace NULL or not 256-byte aligned", name);
+    return fa_attn_run<T>(indptr, cols, f, ldf, rec, out, ldo, n, num_edges, D, drop, ws, ws_bytes, stream);
+}
+
+extern "C" int pglb_fa_attn_csr_f32(const int64_t *indptr, const int64_t *cols, const float *f, int64_t ldf,
+                                    const float *rec, float *out, int64_t ldo, int64_t n, int64_t num_edges, int64_t D,
+                                    void *ws, size_t ws_bytes, void *stream_) {
+    return fa_attn_entry<float>("pglb_fa_attn_csr_f32", indptr, cols, f, ldf, rec, out, ldo, n, num_edges, D, ws,
+                                ws_bytes, stream_, nullptr);
+}
+
+extern "C" int pglb_fa_attn_csr_x16(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
+                                    const float *rec, void *out, int64_t ldo, int64_t n, int64_t num_edges, int64_t D,
+                                    int dtype, void *ws, size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_fa_attn_csr_x16";
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    if (dtype == PGLB_DTYPE_BF16)
+        return fa_attn_entry<__nv_bfloat16>(name, indptr, cols, f, ldf, rec, out, ldo, n, num_edges, D, ws, ws_bytes,
+                                            stream_, nullptr);
+    return fa_attn_entry<__half>(name, indptr, cols, f, ldf, rec, out, ldo, n, num_edges, D, ws, ws_bytes, stream_,
+                                 nullptr);
+}
+
+extern "C" int pglb_fa_attn_drop_csr_f32(const int64_t *indptr, const int64_t *cols, const float *f, int64_t ldf,
+                                         const float *rec, float *out, int64_t ldo, int64_t n, int64_t num_edges,
+                                         int64_t D, float attn_drop, uint64_t seed, uint64_t offset, void *ws,
+                                         size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_fa_attn_drop_csr_f32";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    return fa_attn_entry<float>(name, indptr, cols, f, ldf, rec, out, ldo, n, num_edges, D, ws, ws_bytes, stream_,
+                                &drop);
+}
+
+extern "C" int pglb_fa_attn_drop_csr_x16(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf,
+                                         const float *rec, void *out, int64_t ldo, int64_t n, int64_t num_edges,
+                                         int64_t D, int dtype, float attn_drop, uint64_t seed, uint64_t offset,
+                                         void *ws, size_t ws_bytes, void *stream_) {
+    const char *name = "pglb_fa_attn_drop_csr_x16";
+    if (const int rc = attn_drop_check(name, attn_drop, offset)) return rc;
+    PGLB_CHECK_ARG(dtype == PGLB_DTYPE_BF16 || dtype == PGLB_DTYPE_F16, PGLB_EINVAL, "%s: unknown dtype %d", name,
+                   dtype);
+    const AttnDrop drop = attn_drop_of(attn_drop, seed, offset);
+    if (dtype == PGLB_DTYPE_BF16)
+        return fa_attn_entry<__nv_bfloat16>(name, indptr, cols, f, ldf, rec, out, ldo, n, num_edges, D, ws, ws_bytes,
+                                            stream_, &drop);
+    return fa_attn_entry<__half>(name, indptr, cols, f, ldf, rec, out, ldo, n, num_edges, D, ws, ws_bytes, stream_,
+                                 &drop);
 }
 
 // Send/recv with an edge operand over 16-bit x / out (include/pglb.h): the node-parallel kernel with MODE 1 -- the

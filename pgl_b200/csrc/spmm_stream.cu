@@ -1072,7 +1072,43 @@ int gatv2_attn_run(const int64_t *indptr, const int64_t *cols, const void *f, in
     return launch_gatv2_attn<T, false>(p, attn, AttnDrop{}, stream);
 }
 
+template <typename T>
+bool fa_attn_takes(int64_t D, const void *f, int64_t ldf, const float *rec, int64_t n) {
+    return fa_attn_eligible<T>(D, f, ldf, rec, n);
+}
+
+// Single-pass FAConv aggregation: out[d,:] = sum over the dst-CSR slots j of row d of w_j f[src_j,:], w_j =
+// fa_weight(rec[src_j].x, rec[d].z, rec[src_j].y, rec[d].y) (common.cuh), on spmm_gat5_kernel<kScoreFA>.  rec: [n, 4]
+// float32 node records (g_src, norm, g_dst, 0).  T: element type of f and out; the call is one fa_attn_takes accepts.
+// drop (nullable): the attention-dropout stream, keep bit = head 0 of the 4-head keep word of the slot.
+template <typename T>
+int fa_attn_run(const int64_t *indptr, const int64_t *cols, const void *f, int64_t ldf, const float *rec, void *out,
+                int64_t ldo, int64_t n, int64_t E, int64_t D, const AttnDrop *drop, void *ws, size_t ws_bytes,
+                cudaStream_t stream) {
+    StreamP p{};
+    p.ldy = 1;
+    p.head_dim = (int)D;
+    {
+        const int rc = stream_prepare(p, gat_task_size(E), indptr, cols, f, ldf, out, ldo, n, E, D, PGLB_REDUCE_SUM,
+                                      nullptr, nullptr, nullptr, nullptr, ws, ws_bytes, stream);
+        if (rc) return rc;
+    }
+    p.dyn = dyn_mode(1, p.ntasks);
+    {
+        const int rc = launch_empty_rows<T>(p, stream);
+        if (rc) return rc;
+    }
+    if (drop) return launch_fa_attn<T, true>(p, rec, *drop, stream);
+    return launch_fa_attn<T, false>(p, rec, AttnDrop{}, stream);
+}
+
 // the instantiations the entries in spmm.cu call
+template decltype(fa_attn_takes<float>) fa_attn_takes<float>;
+template decltype(fa_attn_takes<__nv_bfloat16>) fa_attn_takes<__nv_bfloat16>;
+template decltype(fa_attn_takes<__half>) fa_attn_takes<__half>;
+template decltype(fa_attn_run<float>) fa_attn_run<float>;
+template decltype(fa_attn_run<__nv_bfloat16>) fa_attn_run<__nv_bfloat16>;
+template decltype(fa_attn_run<__half>) fa_attn_run<__half>;
 template decltype(gatv2_attn_takes<float>) gatv2_attn_takes<float>;
 template decltype(gatv2_attn_takes<__nv_bfloat16>) gatv2_attn_takes<__nv_bfloat16>;
 template decltype(gatv2_attn_takes<__half>) gatv2_attn_takes<__half>;

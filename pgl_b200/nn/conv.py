@@ -702,7 +702,10 @@ class FAConv(nn.Module):
     """reference pgl/nn/conv.py:1287-1341.  The gate ``tanh(Linear([h_src ; h_dst]))`` splits into
     ``send_uv(h W_top, h W_bot, add)`` (two [N,1] projections instead of an [E, 2D] concat) and the
     weighted sum is ``send_ue_recv(mul, sum)``; the UDF spelling of the reference materialises
-    [E, 2D] + [E, D]."""
+    [E, 2D] + [E, D].  On a ``Graph`` with CUDA features the gate, the norms, the dropout and the weighted sum are one
+    fused pass with a fused backward (``ops.fa_attention``): no [E] tensor; calls those kernels refuse keep the op-by-op
+    route.  The fused route returns the op-by-op route's dtype (torch's promotion of the feature, gate and norm dtypes);
+    16-bit features are aggregated by the 16-bit kernel, whose result is rounded once to the feature dtype first."""
 
     def __init__(self, hidden_size, drop=0.5):
         super().__init__()
@@ -715,6 +718,12 @@ class FAConv(nn.Module):
         d = self.hidden_size
         g_src = feature @ self.gate.weight[:d]
         g_dst = feature @ self.gate.weight[d:] + self.gate.bias
+        if type(graph).__name__ == "Graph" and feature.is_cuda:
+            drop = self.dropout.p if self.training else 0.0
+            output = ops.fa_attention(graph._fwd_csr(), graph._bwd_csr, feature, g_src, g_dst, norm, attn_drop=drop)
+            if output is not None:
+                want = functools.reduce(torch.promote_types, (feature.dtype, g_src.dtype, g_dst.dtype, norm.dtype))
+                return output if output.dtype == want else output.to(want)
         h = torch.tanh(graph.send_uv(g_src, g_dst, "add"))
         alpha = h * graph.send_uv(norm, norm, "mul")
         alpha = self.dropout(alpha)

@@ -2021,6 +2021,138 @@ def gatv2_attention(fwd, bwd, f, attn, negative_slope, out_dtype=None, attn_drop
     return out if out.dtype == res else out.to(res)
 
 
+def _fa_records(g_src, norm, g_dst):
+    """The [N, 4] float32 node records (g_src, norm, g_dst, 0) of pglb_fa_attn_*: one 16-byte bulk copy per slot."""
+    return torch.stack((g_src.float(), norm.float(), g_dst.float(), torch.zeros_like(g_src, dtype=torch.float32)), 1)
+
+
+def _fa_fwd_raw(fwd, f2, rec, drop):
+    """pglb_fa_attn_* on [N, D] rows: out in f2's dtype."""
+    n, D = int(f2.shape[0]), int(f2.shape[1])
+    E = int(fwd["cols"].shape[0])
+    out = torch.empty((n, D), dtype=f2.dtype, device=f2.device)
+    need = ctypes.c_size_t(0)
+    check(lib.pglb_spmm_csr_ws(n, E, D, ctypes.byref(need)))
+    ws = workspace(f2.device, need.value)
+    args = (_ptr(fwd["indptr"]), _ptr(fwd["cols"]), _ptr(f2), f2.stride(0), _ptr(rec), _ptr(out), out.stride(0), n, E,
+            D)
+    dt = (_DTYPE16[f2.dtype],) if f2.dtype in HALF_DTYPES else ()
+    fn = {(False, False): lib.pglb_fa_attn_csr_f32, (False, True): lib.pglb_fa_attn_csr_x16,
+          (True, False): lib.pglb_fa_attn_drop_csr_f32, (True, True): lib.pglb_fa_attn_drop_csr_x16}
+    with torch.cuda.device(f2.device):
+        check(fn[(drop is not None, bool(dt))](*args, *dt, *(drop or ()), _ptr(ws), ws.numel(), _stream()))
+    return out
+
+
+class _FaFused(torch.autograd.Function):
+    """FAConv's self-gated aggregation under autograd (reference pgl/nn/conv.py:1306-1339 differentiated by Paddle over
+    send_uv(add), tanh, send_uv(mul), the product, dropout and send_ue_recv).  Forward = pglb_fa_attn_* (one pass;
+    keeps only N-sized tensors: f2 and the [N, 4] node records, plus (seed, offset)).  Backward = one edge kernel
+    (pglb_fa_bwd_edge_*: weights rebuilt bit for bit, beta and dz per edge, 8 bytes per edge alive only inside the
+    backward) + three aggregations on the existing kernels: grad f = send_ue_recv(G, beta) and grad g_src = segment sum
+    of dz over the src-keyed CSR, grad g_dst = segment sum of dz over the dst-keyed CSR.  16-bit f2 takes the *_x16
+    entries; beta and dz are float32, grad f is aggregated in float32 on the widened G and comes back in f2's dtype,
+    grad g_src / g_dst in their own dtypes.
+    norm is a constant (no gradient)."""
+
+    @staticmethod
+    def forward(ctx, f2, g_src, g_dst, norm, fwd, bwd, drop):
+        rec = _fa_records(g_src, norm, g_dst)
+        out = _fa_fwd_raw(fwd, f2, rec, drop)
+        ctx.meta = (fwd, bwd, drop, g_src.dtype, g_dst.dtype)
+        ctx.save_for_backward(f2, rec)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        fwd, bwd, drop, gs_dtype, gd_dtype = ctx.meta
+        bwd = bwd() if callable(bwd) else bwd
+        f2, rec = ctx.saved_tensors
+        half = f2.dtype in HALF_DTYPES
+        g = _f32_2d(g.to(f2.dtype) if g.dtype != f2.dtype else g, allow16=half)
+        E = int(fwd["cols"].shape[0])
+        n, D = int(f2.shape[0]), int(f2.shape[1])
+        beta = torch.empty((E, 1), dtype=torch.float32, device=g.device)
+        dz = torch.empty((E, 1), dtype=torch.float32, device=g.device)
+        dt = (_DTYPE16[f2.dtype],) if half else ()
+        fn = {(False, False): lib.pglb_fa_bwd_edge_f32, (False, True): lib.pglb_fa_bwd_edge_x16,
+              (True, False): lib.pglb_fa_bwd_edge_drop_f32, (True, True): lib.pglb_fa_bwd_edge_drop_x16}
+        with torch.cuda.device(g.device):
+            check(fn[(drop is not None, half)](
+                _ptr(fwd["rows"]), _ptr(fwd["cols"]), _ptr(fwd["eid"]), _ptr(f2), f2.stride(0), _ptr(rec), _ptr(g),
+                g.stride(0), E, D, *dt, *(drop or ()), _ptr(beta), _ptr(dz), _stream()))
+        gf = gs = gd = None
+        if ctx.needs_input_grad[0]:   # grad f[u] = sum over the out-edges of u of beta[e] G[dst]
+            # 16-bit G is widened and aggregated on the float32 route, then rounded once: on cfg3's graph the 16-bit
+            # edge-operand kernel made the bfloat16 D = 128 training step slower than the op-by-op route (DESIGN 4.18)
+            gf = _spmm_raw(bwd["indptr"], bwd["cols"], g.float() if half else g, n, "sum", eid=bwd["eid"], y2=beta,
+                           y_bcast=BCAST_SCALAR, head_dim=1, msg_op="mul", max_degree=bwd.get("max_degree", -1))
+            gf = gf.to(f2.dtype) if half else gf
+        if ctx.needs_input_grad[1]:   # z = g_src[src] + g_dst[dst]: send_uv(add)'s backward
+            gs = _spmm_raw(bwd["indptr"], bwd["eid"], dz, n, "sum", max_degree=bwd.get("max_degree", -1))
+            gs = gs.reshape(n).to(gs_dtype)
+        if ctx.needs_input_grad[2]:
+            gd = _spmm_raw(fwd["indptr"], fwd["eid"], dz, n, "sum", max_degree=fwd.get("max_degree", -1))
+            gd = gd.reshape(n).to(gd_dtype)
+        return gf, gs, gd, None, None, None, None
+
+
+def fa_attention(fwd, bwd, f, g_src, g_dst, norm, attn_drop=0.0, seed=None, out_dtype=None):
+    """FAConv's self-gated aggregation in one pass:
+    out[d,:] = sum over the in-edges e = (u -> d) of d of keep_e s ((tanh(g_src[u] + g_dst[d]) norm[u]) norm[d]) f[u,:]
+    with a fused backward when autograd needs one (grad f, g_src and g_dst; norm is a constant).  f [N, D]; g_src, g_dst
+    and norm [N] or [N, 1] on one graph (n_dst == N); ``fwd`` is the dst-keyed CSR dict (with ``rows``), ``bwd`` the
+    src-keyed one or a callable returning it.  The result dtype is ``out_dtype``, or by default torch's promotion of
+    f's, g_src's and g_dst's dtypes.  float32 f runs the float32 kernels (g_src, g_dst and norm widened to float32);
+    bfloat16 / float16 f runs the 16-bit kernels when the result dtype is f's (the output is the float32 kernel's on the
+    widened f, rounded once; grad f in f's dtype, grad g_src / g_dst in theirs).  Returns [N, D], or None when the call
+    is outside the kernels (float64, another dtype mix, D > 128 or rows not a multiple of 16 bytes, norm requiring
+    grad, n_dst != N, no edges, attn_drop >= 1, misaligned f, dropout during CUDA-graph capture); the caller then keeps
+    the op-by-op path.
+    ``attn_drop`` in (0, 1): dropout on the edge weights inside the kernels, the keep bit of dst-CSR slot j being head 0
+    of GAT's 4-head keep word, drawn from ``seed`` = (seed, offset), offset a multiple of 4, or by default from the
+    default CUDA generator of f's device (whose offset then advances by 4); kept weights are scaled by 1 / (1 - p).
+    The mask is not nn.Dropout's: only its distribution and its replay from (seed, offset) are promised."""
+    require_cuda(f, g_src, g_dst, norm)
+    if f.dim() != 2:
+        return None
+    n, D = int(f.shape[0]), int(f.shape[1])
+    for t in (g_src, g_dst, norm):
+        if not t.dtype.is_floating_point or t.numel() != n or not (t.dim() == 1 or (t.dim() == 2 and t.shape[1] == 1)):
+            return None
+    if norm.requires_grad:
+        return None
+    half = f.dtype in HALF_DTYPES
+    if torch.float64 in (f.dtype, g_src.dtype, g_dst.dtype, norm.dtype):
+        return None
+    res = _result_dtype(out_dtype, f, g_src, g_dst)
+    if not (f.dtype == torch.float32 or (half and res == f.dtype and
+                                         torch.promote_types(f.dtype, torch.promote_types(g_src.dtype, g_dst.dtype))
+                                         == f.dtype)):
+        return None
+    if D <= 0 or D > 128 or (D * f.element_size()) % 16:
+        return None
+    attn_drop = float(attn_drop)
+    if not 0.0 <= attn_drop < 1.0:
+        return None
+    if attn_drop > 0.0 and torch.cuda.is_current_stream_capturing():
+        return None     # the generator's offset advances on the host: not replayable by a graph
+    if int(fwd["indptr"].shape[0]) - 1 != n or int(fwd["cols"].shape[0]) == 0 or fwd.get("rows") is None:
+        return None
+    f2 = _f32_2d(f, allow16=half)
+    if f2.data_ptr() % 16 or (f2.stride(0) * f2.element_size()) % 16:
+        return None
+    gs, gd, nm = (t.reshape(n) for t in (g_src, g_dst, norm))
+    drop = None
+    if attn_drop > 0.0:
+        drop = (attn_drop,) + (tuple(int(s) for s in seed) if seed is not None else _attn_drop_stream(f2.device))
+    if torch.is_grad_enabled() and (f.requires_grad or g_src.requires_grad or g_dst.requires_grad):
+        out = _FaFused.apply(f2, gs, gd, nm, fwd, bwd, drop)
+    else:
+        out = _fa_fwd_raw(fwd, f2, _fa_records(gs, nm, gd), drop)
+    return out if out.dtype == res else out.to(res)
+
+
 def _aligned16(t):
     """t contiguous with a 16-byte aligned base (rows are then 16-byte aligned for widths % 4 == 0)."""
     t = t.contiguous()
