@@ -212,6 +212,41 @@ int pglb_spmm_narrow_f32(const uint32_t *plan, const int32_t *nz_row, const int3
                          int64_t num_edges, int64_t D, int reduce_op, const float *scale_src, const float *scale_slot,
                          const float *scale_dst, int flags, void *ws, size_t ws_bytes, void *stream);
 
+/* One K-hop propagation step (APPNP, GCNII, SSGCConv, GPRConv; ChebNetII / BernNet recurrences) as one aggregation
+ * with a row epilogue.  For every destination row d, with t[d] the row pglb_spmm_csr_slot_scale_f32 (copy message,
+ * reduce SUM, the same scales) writes -- same route, slot order, hub / cut-row merging, and the same t for rows
+ * without a slot:
+ *   y[d]       = h ? a*t[d] + b*h[d] : a*t[d]
+ *   out[d]     = y[d]
+ *   acc_out[d] = acc_in[d] + cc*y[d]          (when acc_out is given; cc = c_dev ? *c_dev : c)
+ * each product and sum rounded on its own (no FMA contraction): with a = (float)(1 - alpha), b = (float)alpha, h = h0
+ * it is bit for bit torch's `alpha * h0 + (1 - alpha) * propagate(x)`.  c_dev (nullable, device float) lets a caller
+ * take c from a device tensor without a host sync.  Arguments: pglb_spmm_csr_slot_scale_f32's without eid, y, ldy,
+ * y_bcast, head_dim, msg_op and reduce_op, plus
+ *   h [n_dst, ldh] (nullable; may be x itself), acc_in [n_dst, ld_acc_in] and acc_out [n_dst, ld_acc_out] (both or
+ *   neither; acc_out == acc_in with the same stride updates in place).
+ * ws: pglb_spmm_csr_ws(n_dst, E, D).  flags: PGLB_SPMM_L2_HINTS as above.  Refused before any CUDA call:
+ *   PGLB_EINVAL   acc_out without acc_in (or the reverse); out overlapping x, h, acc_in or acc_out; acc_out
+ *                 overlapping x, h, or acc_in other than as the same pointer and stride; scale_slot without scale_src
+ *   PGLB_ESHAPE   ldh, ld_acc_in or ld_acc_out < D
+ *   PGLB_EUNSUPPORTED  PGLB_SPMM_ACCUMULATE; a wide-row shape the copy-sum entry would send to spmm_stream (it has no
+ *                 epilogue); h / acc rows that are not 16-byte aligned where x and out are (the vector kernels). */
+int pglb_propagate_f32(const int64_t *indptr, const int64_t *cols, const float *x, int64_t ldx, float *out, int64_t ldo,
+                       int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t D, const float *scale_src,
+                       const float *scale_slot, const float *scale_dst, float a, float b, const float *h, int64_t ldh,
+                       const float *acc_in, int64_t ld_acc_in, float *acc_out, int64_t ld_acc_out, float c,
+                       const float *c_dev, const uint32_t *cols_packed, int64_t max_degree_hint, int flags, void *ws,
+                       size_t ws_bytes, void *stream);
+/* The same step over pglb_spmm_narrow_f32's plan (reduce SUM): its argument checks, then pglb_propagate_f32's on the
+ * epilogue operands; h / acc rows must be 16-byte aligned (PGLB_EUNSUPPORTED).  t[d] is the row pglb_spmm_narrow_f32
+ * writes.  ws: pglb_spmm_narrow_ws(E, D). */
+int pglb_propagate_narrow_f32(const uint32_t *plan, const int32_t *nz_row, const int32_t *blk_k, const int64_t *indptr,
+                              const float *x, int64_t ldx, float *out, int64_t ldo, int64_t n_dst, int64_t n_src,
+                              int64_t num_edges, int64_t D, const float *scale_src, const float *scale_slot,
+                              const float *scale_dst, float a, float b, const float *h, int64_t ldh,
+                              const float *acc_in, int64_t ld_acc_in, float *acc_out, int64_t ld_acc_out, float c,
+                              const float *c_dev, int flags, void *ws, size_t ws_bytes, void *stream);
+
 /* ------------------------------------------------------------------------------------
  * Edge-parallel ops
  * ---------------------------------------------------------------------------------- */

@@ -61,7 +61,13 @@ _SIGS = {
     "pglb_spmm_narrow_ws": (c_int, [_i64, _i64, POINTER(c_size_t)]),
     "pglb_spmm_narrow_f32": (c_int, [_p, _p, _p, _p, _p, _i64, _p, _i64, _i64, _i64, _i64, _i64, c_int, _p, _p, _p,
                                      c_int, _p, c_size_t, _p]),
-    "pglb_memcpy2d_async": (c_int, [_p, c_size_t, _p, c_size_t, c_size_t, c_size_t, c_int, _p]),
+    "pglb_propagate_f32": (c_int, [_p, _p, _p, _i64, _p, _i64, _i64, _i64, _i64, _i64, _p, _p, _p, ctypes.c_float,
+                                   ctypes.c_float, _p, _i64, _p, _i64, _p, _i64, ctypes.c_float, _p, _p, _i64, c_int,
+                                   _p, c_size_t, _p]),
+    "pglb_propagate_narrow_f32": (c_int, [_p, _p, _p, _p, _p, _i64, _p, _i64, _i64, _i64, _i64, _i64, _p, _p, _p,
+                                          ctypes.c_float, ctypes.c_float, _p, _i64, _p, _i64, _p, _i64,
+                                          ctypes.c_float, _p, c_int, _p, c_size_t, _p]),
+    "pglb_memcpy2d_async": (c_int,[_p, c_size_t, _p, c_size_t, c_size_t, c_size_t, c_int, _p]),
     "pglb_ipc_alloc": (c_int, [c_size_t, POINTER(c_void_p), _p]),
     "pglb_ipc_free": (c_int, [_p]),
     "pglb_ipc_open": (c_int, [_p, POINTER(c_void_p)]),

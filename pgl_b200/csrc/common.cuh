@@ -88,6 +88,52 @@ int radix_sort_u64(uint64_t *keys, uint64_t *vals, uint64_t *keys_alt, uint64_t 
 __device__ __forceinline__ int64_t ld_stream(const int64_t *p) { return __ldcs((const long long *)p); }
 __device__ __forceinline__ int64_t ld_ro(const int64_t *p) { return __ldg((const long long *)p); }
 
+// Row epilogue of pglb_propagate_f32 / pglb_propagate_narrow_f32 (include/pglb.h), read only by the kernel
+// instantiations with PROP = true.  With t the row the plain aggregation would write:
+//   y = a t (+ b h),  out = y,  acc_out = acc_in + c y  (c = *c_dev when c_dev is set)
+// Every product and sum is rounded on its own (no FMA contraction), the order torch's op-by-op hop rounds in.
+struct PropEpi {
+    const float *h;       // nullable [n, ldh]
+    int64_t ldh;
+    const float *acc_in;  // nullable [n, ld_acc_in]; may be acc_out itself (in place)
+    int64_t ld_acc_in;
+    float *acc_out;       // nullable [n, ld_acc_out]
+    int64_t ld_acc_out;
+    float a, b, c;
+    const float *c_dev;   // nullable: device copy of c
+};
+__device__ __forceinline__ float prop_c(const PropEpi &e) { return e.c_dev ? __ldg(e.c_dev) : e.c; }
+// y for one element; hv is read only when e.h is set
+__device__ __forceinline__ float prop_y(const PropEpi &e, float t, float hv) {
+    return e.h ? __fadd_rn(__fmul_rn(e.a, t), __fmul_rn(e.b, hv)) : __fmul_rn(e.a, t);
+}
+__device__ __forceinline__ float4 prop_y4(const PropEpi &e, float4 t, float4 hv) {
+    return make_float4(prop_y(e, t.x, hv.x), prop_y(e, t.y, hv.y), prop_y(e, t.z, hv.z), prop_y(e, t.w, hv.w));
+}
+__device__ __forceinline__ float4 prop_acc4(float4 ai, float c, float4 y) {
+    return make_float4(__fadd_rn(ai.x, __fmul_rn(c, y.x)), __fadd_rn(ai.y, __fmul_rn(c, y.y)),
+                       __fadd_rn(ai.z, __fmul_rn(c, y.z)), __fadd_rn(ai.w, __fmul_rn(c, y.w)));
+}
+// h and acc_in of row r at column c0, loaded when the row opens (row < n_rows, active lanes)
+__device__ __forceinline__ void prop_open4(const PropEpi &e, int64_t r, int64_t n_rows, bool act, int c0, float4 &hv,
+                                           float4 &ai) {
+    if (!act || r >= n_rows) return;
+    if (e.h) hv = __ldg(reinterpret_cast<const float4 *>(e.h + r * e.ldh + c0));
+    if (e.acc_out) ai = *reinterpret_cast<const float4 *>(e.acc_in + r * e.ld_acc_in + c0);
+}
+// the epilogue of a 4-column piece of row r at column c0 (16-byte aligned rows): writes out and acc_out.  acc_in is
+// read with a plain load: in place it is the row acc_out is about to receive.
+__device__ __forceinline__ void prop_store4(const PropEpi &e, float c, float *out, int64_t ldo, int64_t r, int c0,
+                                            float4 t) {
+    const float4 hv = e.h ? __ldg(reinterpret_cast<const float4 *>(e.h + r * e.ldh + c0)) : t;
+    const float4 y = prop_y4(e, t, hv);
+    *reinterpret_cast<float4 *>(out + r * ldo + c0) = y;
+    if (e.acc_out) {
+        const float4 ai = *reinterpret_cast<const float4 *>(e.acc_in + r * e.ld_acc_in + c0);
+        *reinterpret_cast<float4 *>(e.acc_out + r * e.ld_acc_out + c0) = prop_acc4(ai, c, y);
+    }
+}
+
 // 3xTF32 products (linear_tc.cu, rgcn.cu): x*w ~= x_lo*w_hi + x_hi*w_lo + x_hi*w_hi with x_hi = tf32(x),
 // x_lo = tf32(x - x_hi), each term one mma.sync.m16n8k8 accumulating in fp32
 __device__ __forceinline__ uint32_t to_tf32(float v) {

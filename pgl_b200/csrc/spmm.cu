@@ -58,6 +58,7 @@ struct SpmmP {
     unsigned long long *hub_count;
     int64_t *hub_rows;
     int accumulate;  // SUM only: add the previous contents of out before the row epilogue
+    PropEpi epi;     // PROP kernels only (copy sum, float32)
 };
 
 template <int VEC>
@@ -110,7 +111,8 @@ __device__ __forceinline__ float apply_msg(int op, float a, float b) {
 // RK 0: sum / mean;  RK 1: max / min
 // TI / TO: element type of p.x / p.out (float, or the 16-bit type of pglb_spmm_csr_x16; its hub pass 1 writes fp32
 // partials and pass 2 reads them).  Messages are widened to fp32 on load, and each output is rounded once on store.
-template <typename TI, typename TO, int VEC, int G, int ITERS, int MODE, int RK>
+// PROP (TI = TO = float, copy sum): the row closes with p.epi's epilogue (pglb_propagate_f32).
+template <typename TI, typename TO, int VEC, int G, int ITERS, int MODE, int RK, bool PROP = false>
 __device__ __forceinline__ void spmm_csr_body(const SpmmP &p) {
     constexpr int U = (8 / ITERS) < G ? (8 / ITERS) : G;
     const int lane = threadIdx.x & 31;
@@ -168,20 +170,55 @@ __device__ __forceinline__ void spmm_csr_body(const SpmmP &p) {
                 inv_cnt = (float)cnt;
             }
             const float sd = p.scale_dst ? __ldg(p.scale_dst + orow) : 1.0f;
+            if constexpr (PROP) {
+                const float cc = prop_c(p.epi);
 #pragma unroll
-            for (int it = 0; it < ITERS; ++it) {
-                if (!act[it]) continue;
-                float v[VEC];
+                for (int it = 0; it < ITERS; ++it) {
+                    if (!act[it]) continue;
+                    float t[VEC], hv[VEC], y[VEC];
 #pragma unroll
-                for (int j = 0; j < VEC; ++j) {
-                    float a = acc[it][j];
-                    if (deg == 0) a = 0.0f;
-                    if (sizeof(TO) == 4 && p.accumulate) a = __fadd_rn(p.out[orow * p.ldo + col[it] + j], a);
-                    if (p.reduce_op == PGLB_REDUCE_MEAN && deg != 0) a = __fdiv_rn(a, inv_cnt);
-                    if (p.scale_dst) a = __fmul_rn(a, sd);
-                    v[j] = a;
+                    for (int j = 0; j < VEC; ++j) {
+                        float a = acc[it][j];
+                        if (deg == 0) a = 0.0f;
+                        if (p.scale_dst) a = __fmul_rn(a, sd);
+                        t[j] = a;
+                        hv[j] = a;
+                    }
+                    if (p.epi.h) VecIO<VEC>::ld(p.epi.h + orow * p.epi.ldh + col[it], hv);
+#pragma unroll
+                    for (int j = 0; j < VEC; ++j) y[j] = prop_y(p.epi, t[j], hv[j]);
+                    VecIO<VEC>::st(p.out + orow * p.ldo + col[it], y);
+                    if (p.epi.acc_out) {
+                        // plain loads: in place, acc_in is the row this thread is about to overwrite
+                        const float *ai = p.epi.acc_in + orow * p.epi.ld_acc_in + col[it];
+                        float ao[VEC];
+                        if constexpr (VEC == 4) {
+                            const float4 v = *reinterpret_cast<const float4 *>(ai);
+                            ao[0] = v.x; ao[1] = v.y; ao[2] = v.z; ao[3] = v.w;
+                        } else {
+                            ao[0] = *ai;
+                        }
+#pragma unroll
+                        for (int j = 0; j < VEC; ++j) ao[j] = __fadd_rn(ao[j], __fmul_rn(cc, y[j]));
+                        VecIO<VEC>::st(p.epi.acc_out + orow * p.epi.ld_acc_out + col[it], ao);
+                    }
                 }
-                VecIO<VEC>::st(reinterpret_cast<TO *>(p.out) + orow * p.ldo + col[it], v);
+            } else {
+#pragma unroll
+                for (int it = 0; it < ITERS; ++it) {
+                    if (!act[it]) continue;
+                    float v[VEC];
+#pragma unroll
+                    for (int j = 0; j < VEC; ++j) {
+                        float a = acc[it][j];
+                        if (deg == 0) a = 0.0f;
+                        if (sizeof(TO) == 4 && p.accumulate) a = __fadd_rn(p.out[orow * p.ldo + col[it] + j], a);
+                        if (p.reduce_op == PGLB_REDUCE_MEAN && deg != 0) a = __fdiv_rn(a, inv_cnt);
+                        if (p.scale_dst) a = __fmul_rn(a, sd);
+                        v[j] = a;
+                    }
+                    VecIO<VEC>::st(reinterpret_cast<TO *>(p.out) + orow * p.ldo + col[it], v);
+                }
             }
         };
 
@@ -278,9 +315,9 @@ __device__ __forceinline__ void spmm_csr_body(const SpmmP &p) {
     }
 }
 
-template <typename TI, typename TO, int VEC, int G, int ITERS, int MODE, int RK>
+template <typename TI, typename TO, int VEC, int G, int ITERS, int MODE, int RK, bool PROP = false>
 __global__ void __launch_bounds__(kThreads) spmm_csr_kernel(const SpmmP p) {
-    spmm_csr_body<TI, TO, VEC, G, ITERS, MODE, RK>(p);
+    spmm_csr_body<TI, TO, VEC, G, ITERS, MODE, RK, PROP>(p);
 }
 // 4 elements per lane with 2 column iterations (129 <= D <= 256): under __launch_bounds__(kThreads)
 // ptxas holds these at 80 registers and spills 16-32 bytes; a cap of 96 registers instead removes the spills and ran
@@ -427,6 +464,23 @@ static SpmmKernel pick_kernel(const Shape &s, int mode, int rk) {
     return s.vec == 4 ? pick_kernel_v<TI, TO, 4>(s, mode, rk) : pick_kernel_v<TI, TO, 1>(s, mode, rk);
 }
 
+// the float32 copy-sum kernel of shape s with pglb_propagate_f32's row epilogue
+template <int VEC>
+static SpmmKernel pick_prop_kernel_v(const Shape &s) {
+    switch (s.g) {
+        case 4: return spmm_csr_kernel<float, float, VEC, 4, 1, 0, 0, true>;
+        case 8: return spmm_csr_kernel<float, float, VEC, 8, 1, 0, 0, true>;
+        case 16: return spmm_csr_kernel<float, float, VEC, 16, 1, 0, 0, true>;
+        default:
+            if (s.iters == 1) return spmm_csr_kernel<float, float, VEC, 32, 1, 0, 0, true>;
+            if (s.iters == 2) return spmm_csr_kernel<float, float, VEC, 32, 2, 0, 0, true>;
+            return spmm_csr_kernel<float, float, VEC, 32, 4, 0, 0, true>;
+    }
+}
+static SpmmKernel pick_prop_kernel(const Shape &s) {
+    return s.vec == 4 ? pick_prop_kernel_v<4>(s) : pick_prop_kernel_v<1>(s);
+}
+
 struct HubWs {
     unsigned long long *hub_count;  // [1]
     int64_t *total_chunks;          // [1]
@@ -521,6 +575,10 @@ int spmm_v5_run(const int64_t *indptr, const int64_t *cols, const void *x, int64
                 int64_t n_dst, int64_t E, int64_t D, int reduce_op, const float *scale_src, const float *scale_slot,
                 const float *scale_dst, const uint32_t *cols32, int l2_hints, int accumulate, void *ws,
                 size_t ws_bytes, cudaStream_t stream);
+int propagate_v5_run(const int64_t *indptr, const int64_t *cols, const float *x, int64_t ldx, float *out, int64_t ldo,
+                     int64_t n_dst, int64_t E, int64_t D, const float *scale_src, const float *scale_slot,
+                     const float *scale_dst, const uint32_t *cols32, int l2_hints, const PropEpi &epi, void *ws,
+                     size_t ws_bytes, cudaStream_t stream);
 
 // The node-parallel launch sequence behind both entries: spmm_csr kernel over all rows, then, when some row is longer
 // than HUB_T slots, the hub plan and the two hub passes.  E is the element type of x and out.  The main pass reads E
@@ -530,7 +588,8 @@ static int spmm_generic_run(const int64_t *indptr, const int64_t *cols, const in
                             int64_t ldx, const float *y, int64_t ldy, int y_bcast, void *out, int64_t ldo,
                             int64_t n_dst, int64_t num_edges, int64_t D, int64_t head_dim, int msg_op, int reduce_op,
                             const float *scale_src, const float *scale_dst, int64_t max_degree_hint, int accumulate,
-                            bool vec4, void *ws, size_t ws_bytes, cudaStream_t stream) {
+                            bool vec4, void *ws, size_t ws_bytes, cudaStream_t stream,
+                            const PropEpi *epi = nullptr) {
     const Shape s = pick_shape(D, vec4);
     const int mode = (msg_op == PGLB_MSG_COPY) ? 0 : 1;
     const int rk = (reduce_op >= PGLB_REDUCE_MAX) ? 1 : 0;
@@ -574,6 +633,7 @@ static int spmm_generic_run(const int64_t *indptr, const int64_t *cols, const in
     p.hub_count = h.hub_count;
     p.hub_rows = h.hub_rows;
     p.accumulate = accumulate;
+    if (epi) p.epi = *epi;
 
     const int64_t gpb = kThreads / s.g;
     {
@@ -581,7 +641,7 @@ static int spmm_generic_run(const int64_t *indptr, const int64_t *cols, const in
         const int64_t blocks = (tasks + gpb - 1) / gpb;
         PGLB_CHECK_ARG(blocks <= 0x7fffffffLL, PGLB_ESHAPE, "pglb_spmm_csr: grid too large");
         dim3 grid((unsigned)blocks, (unsigned)s.tiles);
-        pick_kernel<E, E>(s, mode, rk)<<<grid, kThreads, 0, stream>>>(p);
+        (epi ? pick_prop_kernel(s) : pick_kernel<E, E>(s, mode, rk))<<<grid, kThreads, 0, stream>>>(p);
         PGLB_LAUNCH_CHECK("spmm_csr_kernel");
     }
     if (need_hub) {
@@ -633,7 +693,7 @@ static int spmm_generic_run(const int64_t *indptr, const int64_t *cols, const in
             int64_t blocks = (h.hub_cap + gpb - 1) / gpb;
             if (blocks > max_blocks) blocks = max_blocks;
             dim3 grid((unsigned)blocks, (unsigned)s.tiles);
-            pick_kernel<float, E>(s, 0, rk)<<<grid, kThreads, 0, stream>>>(p2);
+            (epi ? pick_prop_kernel(s) : pick_kernel<float, E>(s, 0, rk))<<<grid, kThreads, 0, stream>>>(p2);
             PGLB_LAUNCH_CHECK("spmm_csr_kernel(hub pass 2)");
         }
     }
@@ -864,6 +924,43 @@ static int gatv2_score_grad_run(const int64_t *indptr, const int64_t *cols, cons
     return PGLB_OK;
 }
 
+// [p, p + extent) of an n-row matrix of D floats per row at stride ld
+static bool overlaps(const void *p, int64_t n, int64_t ld, const void *q, int64_t m, int64_t ldq, int64_t D) {
+    if (!p || !q || n <= 0 || m <= 0) return false;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q);
+    const uintptr_t ae = a + (uintptr_t)(((n - 1) * ld + D) * 4), be = b + (uintptr_t)(((m - 1) * ldq + D) * 4);
+    return a < be && b < ae;
+}
+
+int prop_check_args(const char *entry, const void *x, int64_t ldx, int64_t n_src, const void *out, int64_t ldo,
+                    int64_t n_dst, int64_t D, const float *h, int64_t ldh, const float *acc_in, int64_t ld_acc_in,
+                    const float *acc_out, int64_t ld_acc_out, int flags) {
+    PGLB_CHECK_ARG(!(flags & PGLB_SPMM_ACCUMULATE), PGLB_EUNSUPPORTED, "%s: PGLB_SPMM_ACCUMULATE is not taken", entry);
+    PGLB_CHECK_ARG(!acc_out == !acc_in, PGLB_EINVAL, "%s: acc_in and acc_out come together", entry);
+    PGLB_CHECK_ARG((!h || ldh >= D) && (!acc_in || ld_acc_in >= D) && (!acc_out || ld_acc_out >= D), PGLB_ESHAPE,
+                   "%s: leading dimension of h / acc smaller than D", entry);
+    if (n_dst == 0 || D == 0) return PGLB_OK;
+    // rows of out and acc_out are written while x and h are gathered and acc_in is read: only acc_out == acc_in (the
+    // same rows at the same stride) may share memory
+    PGLB_CHECK_ARG(!overlaps(out, n_dst, ldo, x, n_src, ldx, D) && !overlaps(out, n_dst, ldo, h, n_dst, ldh, D) &&
+                       !overlaps(out, n_dst, ldo, acc_in, n_dst, ld_acc_in, D) &&
+                       !overlaps(out, n_dst, ldo, acc_out, n_dst, ld_acc_out, D),
+                   PGLB_EINVAL, "%s: out overlaps x, h or acc", entry);
+    PGLB_CHECK_ARG(!overlaps(acc_out, n_dst, ld_acc_out, x, n_src, ldx, D) &&
+                       !overlaps(acc_out, n_dst, ld_acc_out, h, n_dst, ldh, D),
+                   PGLB_EINVAL, "%s: acc_out overlaps x or h", entry);
+    PGLB_CHECK_ARG(!overlaps(acc_out, n_dst, ld_acc_out, acc_in, n_dst, ld_acc_in, D) ||
+                       (acc_out == acc_in && ld_acc_out == ld_acc_in),
+                   PGLB_EINVAL, "%s: acc_out overlaps acc_in other than in place", entry);
+    return PGLB_OK;
+}
+
+// the 16-byte row accesses of the vector kernels' epilogues
+bool prop_rows16(const PropEpi &e) {
+    return (!e.h || (aligned16(e.h) && e.ldh % 4 == 0)) && (!e.acc_in || (aligned16(e.acc_in) && e.ld_acc_in % 4 == 0)) &&
+           (!e.acc_out || (aligned16(e.acc_out) && e.ld_acc_out % 4 == 0));
+}
+
 }  // namespace pglb
 
 using namespace pglb;
@@ -958,6 +1055,43 @@ extern "C" int pglb_spmm_csr_slot_scale_f32(const int64_t *indptr, const int64_t
     return spmm_generic_run<float>(indptr, cols, eid, x, ldx, y, ldy, y_bcast, out, ldo, n_dst, num_edges, D, head_dim,
                                    msg_op, reduce_op, scale_src, scale_dst, max_degree_hint, accumulate, vec4, ws,
                                    ws_bytes, stream);
+}
+
+extern "C" int pglb_propagate_f32(const int64_t *indptr, const int64_t *cols, const float *x, int64_t ldx, float *out,
+                                  int64_t ldo, int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t D,
+                                  const float *scale_src, const float *scale_slot, const float *scale_dst, float a,
+                                  float b, const float *h, int64_t ldh, const float *acc_in, int64_t ld_acc_in,
+                                  float *acc_out, int64_t ld_acc_out, float c, const float *c_dev,
+                                  const uint32_t *cols_packed, int64_t max_degree_hint, int flags, void *ws,
+                                  size_t ws_bytes, void *stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    PGLB_CHECK_ARG(!scale_slot || scale_src, PGLB_EINVAL, "pglb_propagate_f32: scale_slot needs scale_src");
+    {
+        int rc = spmm_check_args("pglb_propagate_f32", indptr, x, ldx, out, ldo, n_dst, n_src, num_edges, D,
+                                 PGLB_REDUCE_SUM);
+        if (rc) return rc;
+        rc = prop_check_args("pglb_propagate_f32", x, ldx, n_src, out, ldo, n_dst, D, h, ldh, acc_in, ld_acc_in,
+                             acc_out, ld_acc_out, flags);
+        if (rc) return rc;
+    }
+    if (n_dst == 0 || D == 0) return PGLB_OK;
+    const PropEpi e{h, ldh, acc_in, ld_acc_in, acc_out, ld_acc_out, a, b, c, c_dev};
+    // the route pglb_spmm_csr_slot_scale_f32 takes for copy sum, so the row sums t are the same
+    const bool vec4 = (D % 4 == 0) && (ldx % 4 == 0) && (ldo % 4 == 0) && aligned16(x) && aligned16(out);
+    PGLB_CHECK_ARG(!vec4 || prop_rows16(e), PGLB_EUNSUPPORTED,
+                   "pglb_propagate_f32: h / acc rows must be 16-byte aligned like x and out");
+    if (vec4 && D > 64 && num_edges > 0) {
+        PGLB_CHECK_ARG(v5_eligible<float>(cols, cols_packed, x, ldx, out, ldo, n_src, num_edges, D, PGLB_REDUCE_SUM),
+                       PGLB_EUNSUPPORTED, "pglb_propagate_f32: this wide-row shape takes spmm_stream, which has no "
+                       "epilogue (identity columns, ids or rows past 2^31)");
+        PGLB_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 255u) == 0, PGLB_EWORKSPACE,
+                       "pglb_propagate_f32: workspace must be 256-byte aligned");
+        return propagate_v5_run(indptr, cols, x, ldx, out, ldo, n_dst, num_edges, D, scale_src, scale_slot, scale_dst,
+                                cols_packed, (flags & PGLB_SPMM_L2_HINTS) ? 1 : 0, e, ws, ws_bytes, stream);
+    }
+    return spmm_generic_run<float>(indptr, cols, nullptr, x, ldx, nullptr, 0, 0, out, ldo, n_dst, num_edges, D, 1,
+                                   PGLB_MSG_COPY, PGLB_REDUCE_SUM, scale_src, scale_dst, max_degree_hint, 0, vec4, ws,
+                                   ws_bytes, stream, &e);
 }
 
 extern "C" int pglb_spmm_csr_x16(const int64_t *indptr, const int64_t *cols, const void *x, int64_t ldx, void *out,

@@ -683,9 +683,10 @@ __global__ void __launch_bounds__(StreamCfg<ITERS>::kThreads) spmm_stream_kernel
 }
 
 // One warp per task that owns a cut row: out[r] = epilogue(tail(t) (+) head(t+1) (+) ...).  The partials are fp32;
-// TO is the element type of out (a 16-bit out is rounded once, on the store).
-template <typename TO, int ITERS, int RK>
-__global__ void __launch_bounds__(256) spmm_stream_fixup_kernel(const StreamP p) {
+// TO is the element type of out (a 16-bit out is rounded once, on the store).  PROP (float, copy sum): the row closes
+// with epi's epilogue.
+template <typename TO, int ITERS, int RK, bool PROP>
+__device__ __forceinline__ void spmm_stream_fixup_body(const StreamP &p, const PropEpi &epi) {
     const int lane = threadIdx.x & 31;
     const int64_t t = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (t >= p.ntasks) return;
@@ -740,11 +741,21 @@ __global__ void __launch_bounds__(256) spmm_stream_fixup_kernel(const StreamP p)
             acc.x = __fmul_rn(acc.x, sd); acc.y = __fmul_rn(acc.y, sd);
             acc.z = __fmul_rn(acc.z, sd); acc.w = __fmul_rn(acc.w, sd);
         }
-        if constexpr (sizeof(TO) == 4)
+        if constexpr (PROP)
+            prop_store4(epi, prop_c(epi), p.out, p.ldo, r, c, acc);
+        else if constexpr (sizeof(TO) == 4)
             *reinterpret_cast<float4 *>(p.out + r * p.ldo + c) = acc;
         else
             *reinterpret_cast<uint2 *>(reinterpret_cast<TO *>(p.out) + r * p.ldo + c) = round4<TO>(acc);
     }
+}
+template <typename TO, int ITERS, int RK>
+__global__ void __launch_bounds__(256) spmm_stream_fixup_kernel(const StreamP p) {
+    spmm_stream_fixup_body<TO, ITERS, RK, false>(p, PropEpi{});
+}
+// the fix-up of pglb_propagate_*'s cut rows (float32, one float4 per lane)
+__global__ void __launch_bounds__(256) spmm_stream_fixup_prop_kernel(const StreamP p, const PropEpi epi) {
+    spmm_stream_fixup_body<float, 1, 0, true>(p, epi);
 }
 
 // Fused-GAT fix-up: merge the (acc, m, l) partials of a cut row: M = max m_i,
@@ -825,6 +836,27 @@ __global__ void __launch_bounds__(256) empty_rows_kernel(const int64_t *__restri
     }
 }
 
+// Rows without a slot under pglb_propagate_*'s epilogue: t = 0, the value empty_rows_kernel writes (float32 rows,
+// D % 4 == 0, 16-byte aligned)
+__global__ void __launch_bounds__(256) empty_rows_prop_kernel(const int64_t *__restrict__ indptr, int64_t n_rows, int D,
+                                                              float *__restrict__ out, int64_t ldo, const PropEpi epi) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const float cc = prop_c(epi);
+    for (int64_t r0 = warp * 32; r0 < n_rows; r0 += nwarps * 32) {
+        const int64_t r = r0 + lane;
+        bool empty = false;
+        if (r < n_rows) empty = ld_ro(indptr + r + 1) == ld_ro(indptr + r);
+        unsigned mask = __ballot_sync(0xffffffffu, empty);
+        while (mask) {
+            const int i = __ffs(mask) - 1;
+            mask &= mask - 1;
+            for (int c = lane * 4; c < D; c += 128) prop_store4(epi, cc, out, ldo, r0 + i, c, make_float4(0.f, 0.f, 0.f, 0.f));
+        }
+    }
+}
+
 template <typename TO>
 static int launch_empty_rows(const StreamP &p, cudaStream_t stream) {
     if (p.accumulate && !p.scale_dst) return PGLB_OK;  // out_prev + 0 unchanged
@@ -835,6 +867,16 @@ static int launch_empty_rows(const StreamP &p, cudaStream_t stream) {
     empty_rows_kernel<TO><<<(unsigned)blocks, 256, 0, stream>>>(p.indptr, p.n_rows, p.D, p.out, p.ldo,
                                                                p.scale_dst, p.accumulate);
     PGLB_LAUNCH_CHECK("empty_rows_kernel");
+    return PGLB_OK;
+}
+
+static int launch_empty_rows_prop(const StreamP &p, const PropEpi &epi, cudaStream_t stream) {
+    int64_t blocks = (p.n_rows + 255) / 256;
+    const int64_t cap = (int64_t)sm_count() * 8;
+    if (blocks > cap) blocks = cap;
+    if (blocks < 1) blocks = 1;
+    empty_rows_prop_kernel<<<(unsigned)blocks, 256, 0, stream>>>(p.indptr, p.n_rows, p.D, p.out, p.ldo, epi);
+    PGLB_LAUNCH_CHECK("empty_rows_prop_kernel");
     return PGLB_OK;
 }
 
@@ -1040,6 +1082,27 @@ int spmm_v5_run(const int64_t *indptr, const int64_t *cols, const void *x, int64
     return launch_v5<T>(p, cols32 != nullptr && cols != nullptr && l2_hints != 0, stream);
 }
 
+// pglb_propagate_f32 on the calls spmm_v5_run<float> takes with reduce_op SUM: the same task plan and kernel geometry,
+// every row closed with epi's epilogue (empty rows by empty_rows_prop_kernel, cut rows by the fix-up)
+int propagate_v5_run(const int64_t *indptr, const int64_t *cols, const float *x, int64_t ldx, float *out, int64_t ldo,
+                     int64_t n_dst, int64_t E, int64_t D, const float *scale_src, const float *scale_slot,
+                     const float *scale_dst, const uint32_t *cols32, int l2_hints, const PropEpi &epi, void *ws,
+                     size_t ws_bytes, cudaStream_t stream) {
+    StreamP p{};
+    p.head_dim = 1;
+    {
+        const int rc = stream_prepare(p, stream_task_size(E), indptr, cols, x, ldx, out, ldo, n_dst, E, D,
+                                      PGLB_REDUCE_SUM, scale_src, scale_slot, scale_dst, cols32, ws, ws_bytes, stream);
+        if (rc) return rc;
+    }
+    p.dyn = dyn_mode(0, p.ntasks);
+    {
+        const int rc = launch_empty_rows_prop(p, epi, stream);
+        if (rc) return rc;
+    }
+    return launch_v5<float, true>(p, cols32 != nullptr && cols != nullptr && l2_hints != 0, stream, &epi);
+}
+
 template <typename T>
 bool gatv2_attn_takes(int64_t D, int64_t head_dim, float slope, const void *f, int64_t ldf, const float *attn,
                       int64_t n_src) {
@@ -1180,8 +1243,15 @@ static int64_t narrow2_task_size(int64_t E, int64_t D) {
 size_t narrow2_ws_bytes(int64_t E, int64_t D) { return stream_layout(nullptr, E, D, narrow2_task_size(E, D)).bytes; }
 
 template <int L>
-static void launch_narrow2(const NarrowP &p, int sc, bool hot, unsigned blocks, cudaStream_t stream) {
+static void launch_narrow2(const NarrowP &p, int sc, bool hot, bool prop, unsigned blocks, cudaStream_t stream) {
 #define PGLB_N2K(SC, MN, HT) spmm_narrow2_kernel<L, SC, MN, HT><<<blocks, kNarrowWarps * 32, 0, stream>>>(p)
+#define PGLB_N2P(SC, HT) spmm_narrow2_kernel<L, SC, false, HT, true><<<blocks, kNarrowWarps * 32, 0, stream>>>(p)
+    if (prop) {  // pglb_propagate_narrow_f32: sum
+        if (sc == 1) hot ? PGLB_N2P(1, true) : PGLB_N2P(1, false);
+        else if (sc == 2) hot ? PGLB_N2P(2, true) : PGLB_N2P(2, false);
+        else hot ? PGLB_N2P(0, true) : PGLB_N2P(0, false);
+        return;
+    }
     if (p.mean) {  // mean (GraphSAGE): no L2 hints
         if (sc == 1) PGLB_N2K(1, true, false);
         else if (sc == 2) PGLB_N2K(2, true, false);
@@ -1198,12 +1268,14 @@ static void launch_narrow2(const NarrowP &p, int sc, bool hot, unsigned blocks, 
         else PGLB_N2K(0, false, false);
     }
 #undef PGLB_N2K
+#undef PGLB_N2P
 }
 
+// epi (nullable, sum only): pglb_propagate_narrow_f32's row epilogue
 int narrow2_run(const uint32_t *plan, const int32_t *nz_row, const int32_t *blk_k, const int64_t *indptr, const float *x,
                 int64_t ldx, float *out, int64_t ldo, int64_t n_dst, int64_t E, int64_t D, int reduce_op,
                 const float *scale_src, const float *sval, const float *scale_dst, int hot, void *ws, size_t ws_bytes,
-                cudaStream_t stream) {
+                cudaStream_t stream, const PropEpi *epi = nullptr) {
     const int64_t T = narrow2_task_size(E, D);
     StreamWs w = stream_layout(ws, E, D, T);
     PGLB_CHECK_ARG(ws != nullptr && ws_bytes >= w.bytes, PGLB_EWORKSPACE,
@@ -1243,20 +1315,24 @@ int narrow2_run(const uint32_t *plan, const int32_t *nz_row, const int32_t *blk_
     sp.partial = w.partial;
     sp.dpad = w.dpad;
     sp.tail_row = w.tail_row;
+    if (epi) p.epi = *epi;
     {
-        const int rc = launch_empty_rows<float>(sp, stream);
+        const int rc = epi ? launch_empty_rows_prop(sp, *epi, stream) : launch_empty_rows<float>(sp, stream);
         if (rc) return rc;
     }
     const int64_t blocks = (p.ntasks + kNarrowWarps - 1) / kNarrowWarps;
     PGLB_CHECK_ARG(blocks <= 0x7fffffffLL, PGLB_ESHAPE, "spmm_narrow2: grid too large");
     const int lpr = narrow2_lpr(D);
     const int sc = sval ? 2 : (scale_src ? 1 : 0);
-    if (lpr == 4) launch_narrow2<4>(p, sc, hot != 0, (unsigned)blocks, stream);
-    else if (lpr == 8) launch_narrow2<8>(p, sc, hot != 0, (unsigned)blocks, stream);
-    else launch_narrow2<16>(p, sc, hot != 0, (unsigned)blocks, stream);
+    if (lpr == 4) launch_narrow2<4>(p, sc, hot != 0, epi != nullptr, (unsigned)blocks, stream);
+    else if (lpr == 8) launch_narrow2<8>(p, sc, hot != 0, epi != nullptr, (unsigned)blocks, stream);
+    else launch_narrow2<16>(p, sc, hot != 0, epi != nullptr, (unsigned)blocks, stream);
     PGLB_LAUNCH_CHECK("spmm_narrow2_kernel");
     const int64_t fblocks = (p.ntasks * 32 + 255) / 256;
-    spmm_stream_fixup_kernel<float, 1, 0><<<(unsigned)fblocks, 256, 0, stream>>>(sp);
+    if (epi)
+        spmm_stream_fixup_prop_kernel<<<(unsigned)fblocks, 256, 0, stream>>>(sp, *epi);
+    else
+        spmm_stream_fixup_kernel<float, 1, 0><<<(unsigned)fblocks, 256, 0, stream>>>(sp);
     PGLB_LAUNCH_CHECK("spmm_stream_fixup_kernel");
     return PGLB_OK;
 }
@@ -1366,6 +1442,14 @@ extern "C" int pglb_debug_task_trace(void *buffer, int64_t capacity_tasks) {
     return PGLB_OK;
 }
 
+namespace pglb {
+// spmm.cu: pglb_propagate_*'s checks of the epilogue operands
+int prop_check_args(const char *entry, const void *x, int64_t ldx, int64_t n_src, const void *out, int64_t ldo,
+                    int64_t n_dst, int64_t D, const float *h, int64_t ldh, const float *acc_in, int64_t ld_acc_in,
+                    const float *acc_out, int64_t ld_acc_out, int flags);
+bool prop_rows16(const PropEpi &e);
+}  // namespace pglb
+
 extern "C" int pglb_spmm_narrow_ws(int64_t num_edges, int64_t D, size_t *ws_bytes) {
     PGLB_CHECK_ARG(ws_bytes != nullptr && num_edges >= 0 && D > 0, PGLB_EINVAL, "pglb_spmm_narrow_ws: bad argument");
     *ws_bytes = narrow2_ws_bytes(num_edges, D);
@@ -1389,4 +1473,33 @@ extern "C" int pglb_spmm_narrow_f32(const uint32_t *plan, const int32_t *nz_row,
     PGLB_CHECK_ARG(n_src < 0x40000000LL && ldx * 4 < 0xffffffffLL, PGLB_ESHAPE, "pglb_spmm_narrow_f32: n_src < 2^30 needed");
     return narrow2_run(plan, nz_row, blk_k, indptr, x, ldx, out, ldo, n_dst, num_edges, D, reduce_op, scale_src, scale_slot,
                        scale_dst, flags & PGLB_SPMM_L2_HINTS, ws, ws_bytes, stream);
+}
+
+extern "C" int pglb_propagate_narrow_f32(const uint32_t *plan, const int32_t *nz_row, const int32_t *blk_k,
+                                         const int64_t *indptr, const float *x, int64_t ldx, float *out, int64_t ldo,
+                                         int64_t n_dst, int64_t n_src, int64_t num_edges, int64_t D,
+                                         const float *scale_src, const float *scale_slot, const float *scale_dst,
+                                         float a, float b, const float *h, int64_t ldh, const float *acc_in,
+                                         int64_t ld_acc_in, float *acc_out, int64_t ld_acc_out, float c,
+                                         const float *c_dev, int flags, void *ws, size_t ws_bytes, void *stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    PGLB_CHECK_ARG(n_dst > 0 && n_src > 0 && num_edges > 0, PGLB_EINVAL, "pglb_propagate_narrow_f32: empty problem");
+    PGLB_CHECK_ARG(D >= 4 && D <= 64 && D % 4 == 0, PGLB_ESHAPE,
+                   "pglb_propagate_narrow_f32: D must be 4..64, a multiple of 4");
+    PGLB_CHECK_ARG(plan && nz_row && blk_k && indptr && x && out, PGLB_EINVAL, "pglb_propagate_narrow_f32: NULL pointer");
+    PGLB_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (ldx % 4) == 0 &&
+                       (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (ldo % 4) == 0,
+                   PGLB_ESHAPE, "pglb_propagate_narrow_f32: x / out rows must be 16-byte aligned");
+    PGLB_CHECK_ARG(n_src < 0x40000000LL && ldx * 4 < 0xffffffffLL, PGLB_ESHAPE,
+                   "pglb_propagate_narrow_f32: n_src < 2^30 needed");
+    {
+        const int rc = prop_check_args("pglb_propagate_narrow_f32", x, ldx, n_src, out, ldo, n_dst, D, h, ldh, acc_in,
+                                       ld_acc_in, acc_out, ld_acc_out, flags);
+        if (rc) return rc;
+    }
+    const PropEpi e{h, ldh, acc_in, ld_acc_in, acc_out, ld_acc_out, a, b, c, c_dev};
+    PGLB_CHECK_ARG(prop_rows16(e), PGLB_EUNSUPPORTED,
+                   "pglb_propagate_narrow_f32: h / acc rows must be 16-byte aligned like x and out");
+    return narrow2_run(plan, nz_row, blk_k, indptr, x, ldx, out, ldo, n_dst, num_edges, D, PGLB_REDUCE_SUM, scale_src,
+                       scale_slot, scale_dst, flags & PGLB_SPMM_L2_HINTS, ws, ws_bytes, stream, &e);
 }

@@ -68,6 +68,17 @@ def _propagate(graph, feature, norm):
     return feature
 
 
+def _propagate_fused(graph, feature, norm, fallback, **kw):
+    """One K-hop step ``a * _propagate(graph, feature, norm) (+ b * h)`` (and ``acc + c * y``) as one aggregation with a
+    row epilogue (``ops.propagate``): bit for bit the op-by-op hop in float32.  Where that route declines (not a plain
+    Graph, a feature or norm it does not take), ``fallback()`` runs the layer's op-by-op hop unchanged."""
+    out = None
+    if type(graph).__name__ == "Graph" and norm is not None and isinstance(feature, torch.Tensor) \
+            and feature.dim() == 2 and graph._n == feature.shape[0]:
+        out = ops.propagate(feature, graph._fwd_csr(), graph._bwd_csr, norm, **kw)
+    return fallback() if out is None else out
+
+
 def _with_self_loops(graph):
     """reference conv.py:474-484: drop the existing self loops, prepend one per node."""
     edges = graph.edges
@@ -339,9 +350,14 @@ class APPNP(nn.Module):
         if norm is None:
             norm = GF.degree_norm(graph)
         h0 = feature
-        for _ in range(self.k_hop):
+
+        def hop(feature):
             feature = _propagate(graph, feature, norm)
-            feature = self.alpha * h0 + (1 - self.alpha) * feature
+            return self.alpha * h0 + (1 - self.alpha) * feature
+
+        for _ in range(self.k_hop):
+            feature = _propagate_fused(graph, feature, norm, functools.partial(hop, feature),
+                                       a=1 - self.alpha, b=self.alpha, h=h0)
         return feature
 
 
@@ -395,9 +411,15 @@ class GPRConv(nn.Module):
         if norm is None:
             norm = GF.degree_norm(graph)
         hidden = feature * self.temp[0]
-        for k in range(self.k_hop):
+
+        def hop(feature, hidden, k):
             feature = _propagate(graph, feature, norm)
-            hidden = hidden + self.temp[k + 1] * feature
+            return feature, hidden + self.temp[k + 1] * feature
+
+        for k in range(self.k_hop):
+            # temp[k + 1] is read on the device: no host sync per hop
+            feature, hidden = _propagate_fused(graph, feature, norm, functools.partial(hop, feature, hidden, k),
+                                               acc=hidden, c=self.temp[k + 1])
         return hidden
 
 
@@ -423,13 +445,17 @@ class GCNII(nn.Module):
         for i in range(self.k_hop):
             beta_i = _math.log(1.0 * self.lambda_l / (i + 1) + 1)
             feature = self.drop_fn(feature)
-            feature = _propagate(graph, feature, norm)
-            feature = self.alpha * h0 + (1 - self.alpha) * feature
+            feature = _propagate_fused(graph, feature, norm, functools.partial(self._hop, graph, feature, norm, h0),
+                                       a=1 - self.alpha, b=self.alpha, h=h0)
             feature_transed = self.mlps[i](feature)
             feature = beta_i * feature_transed + (1 - beta_i) * feature
             if self.activation is not None:
                 feature = self.activation(feature)
         return feature
+
+    def _hop(self, graph, feature, norm, h0):
+        feature = _propagate(graph, feature, norm)
+        return self.alpha * h0 + (1 - self.alpha) * feature
 
 
 class TransformerConv(nn.Module):
@@ -660,9 +686,15 @@ class SSGCConv(_KHopCached):
         norm = GF.degree_norm(graph)
         ori_feature = feature
         sum_feature = feature
-        for _ in range(self.k_hop):
+
+        def hop(feature, sum_feature):
             feature = (1 - self.alpha) * _propagate(graph, feature, norm)
-            sum_feature = sum_feature + feature
+            return feature, sum_feature + feature
+
+        for k in range(self.k_hop):
+            # after the first hop the running sum is a buffer of this call's own, updated in place
+            feature, sum_feature = _propagate_fused(graph, feature, norm, functools.partial(hop, feature, sum_feature),
+                                                    a=1 - self.alpha, acc=sum_feature, inplace_acc=k > 0)
         return sum_feature / self.k_hop + self.alpha * ori_feature
 
     def forward(self, graph, feature):

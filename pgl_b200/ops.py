@@ -1036,6 +1036,162 @@ def aggregate_copy(x, fwd, n_dst, reduce_op="sum", bwd=None, scale_src=None, sca
     return out.reshape((n_dst,) + tuple(shape[1:]))
 
 
+_EUNSUPPORTED = -4   # PGLB_EUNSUPPORTED
+
+
+def _rows16(t):
+    return t.data_ptr() % 16 == 0 and t.stride(0) % 4 == 0
+
+
+def _propagate_raw(csr, x2, scale, a, b, h, acc, c, acc_out):
+    """One pglb_propagate_*_f32 call on the route _spmm_raw takes for x2 with scale_src = scale_dst = scale: the
+    narrow plan when _spmm_raw would use it, else pglb_propagate_f32 with the same packed ids and per-slot scale.
+    c: a float, or a one-element float32 CUDA tensor read on the device.  acc_out: None, acc itself (in place) or a
+    fresh [N, D] tensor.  Returns the output, or None when the entry refuses the call (PGLB_EUNSUPPORTED)."""
+    dev = x2.device
+    n, D = int(x2.shape[0]), int(x2.shape[1])
+    E = int(csr["cols"].shape[0])
+    out = torch.empty((n, D), dtype=torch.float32, device=dev)
+    c_dev = c if isinstance(c, torch.Tensor) else None
+    c_val = 0.0 if c_dev is not None else float(c)
+    epi = (ctypes.c_float(a), ctypes.c_float(b), _ptr(h), h.stride(0) if h is not None else 0, _ptr(acc),
+           acc.stride(0) if acc is not None else 0, _ptr(acc_out), acc_out.stride(0) if acc_out is not None else 0,
+           ctypes.c_float(c_val), _ptr(c_dev))
+    packed = _packed_of(csr, x2)
+    indptr = csr["indptr"]
+    if isinstance(packed, NarrowPlan):
+        if _rows16(x2) and n < (1 << 30):
+            need = ctypes.c_size_t(0)
+            check(lib.pglb_spmm_narrow_ws(E, D, ctypes.byref(need)))
+            ws = workspace(dev, need.value)
+            sval = packed.slot_scale(scale) if (NARROW_SLOT_SCALE and packed.slot_scale is not None) else None
+            with torch.cuda.device(dev):
+                rc = lib.pglb_propagate_narrow_f32(_ptr(packed.plan), _ptr(packed.nz_row), _ptr(packed.blk_k),
+                                                   _ptr(indptr), _ptr(x2), x2.stride(0), _ptr(out), out.stride(0), n,
+                                                   n, E, D, _ptr(scale), _ptr(sval), _ptr(scale), *epi,
+                                                   2 if packed.hints else 0, _ptr(ws), ws.numel(), _stream())
+            if rc == _EUNSUPPORTED:
+                return None
+            check(rc)
+            return out
+        packed = None
+    need = ctypes.c_size_t(0)
+    check(lib.pglb_spmm_csr_ws(n, E, D, ctypes.byref(need)))
+    ws = workspace(dev, need.value)
+    sslot = packed.slot_scale(scale) if getattr(packed, "slot_scale", None) is not None else None
+    flags = 2 if (packed is not None and packed[1]) else 0
+    with torch.cuda.device(dev):
+        rc = lib.pglb_propagate_f32(_ptr(indptr), _ptr(csr["cols"]), _ptr(x2), x2.stride(0), _ptr(out),
+                                    out.stride(0), n, n, E, D, _ptr(scale), _ptr(sslot), _ptr(scale), *epi,
+                                    _ptr(packed[0]) if packed is not None else None,
+                                    int(csr.get("max_degree", -1)), flags, _ptr(ws), ws.numel(), _stream())
+    if rc == _EUNSUPPORTED:
+        return None
+    check(rc)
+    return out
+
+
+class _Propagate(torch.autograd.Function):
+    """y = a * (scale * A (scale * x)) (+ b * h), acc_out = acc + c * y as one aggregation (pglb_propagate_f32).
+    Backward: g_tot = g_y + c g_acc; g_x is one pglb_propagate_f32 call on the reverse CSR with a and the scales
+    swapped (one shared scale here); g_h = b g_tot; g_acc passes through; g_c = sum(g_acc * y).  No atomics: the
+    gradients are the same from run to run."""
+
+    @staticmethod
+    def forward(ctx, x2, h, acc, c, fwd, bwd, scale, a, b):
+        acc_out = torch.empty_like(acc) if acc is not None else None
+        y = _propagate_raw(fwd, x2, scale, a, b, h, acc, c, acc_out)
+        if y is None:
+            raise RuntimeError("pgl_b200: pglb_propagate_f32 refused a call ops.propagate accepted")
+        ctx.bwd, ctx.scale, ctx.a, ctx.b, ctx.c = bwd, scale, a, b, c
+        ctx.c_grad = isinstance(c, torch.Tensor) and ctx.needs_input_grad[3]
+        if ctx.c_grad:
+            ctx.save_for_backward(y)
+        return y if acc is None else (y, acc_out)
+
+    @staticmethod
+    def backward(ctx, g_y, g_acc=None):
+        c = ctx.c
+        g_tot = g_y
+        if g_acc is not None:
+            g_tot = torch.addcmul(g_y, g_acc, c) if isinstance(c, torch.Tensor) else torch.add(g_y, g_acc, alpha=c)
+        g_tot = g_tot.contiguous()
+        g_x = g_h = g_c = None
+        if ctx.needs_input_grad[0]:
+            bwd = ctx.bwd() if callable(ctx.bwd) else ctx.bwd
+            if bwd is None:
+                raise RuntimeError("pgl_b200: backward of this propagation needs the reverse CSR")
+            g_x = _propagate_raw(bwd, g_tot, ctx.scale, ctx.a, 0.0, None, None, 1.0, None)
+            if g_x is None:
+                raise RuntimeError("pgl_b200: pglb_propagate_f32 refused the backward of an accepted call")
+        if ctx.needs_input_grad[1]:
+            g_h = torch.mul(g_tot, ctx.b)
+        if ctx.c_grad:
+            (y,) = ctx.saved_tensors
+            g_c = (g_acc * y).sum().reshape(c.shape) if g_acc is not None else torch.zeros_like(c)
+        return g_x, g_h, g_acc, g_c, None, None, None, None, None
+
+
+def _propagate_declines(x, n, others, scale):
+    if not isinstance(x, torch.Tensor) or not x.is_cuda or x.dtype != torch.float32 or x.dim() != 2:
+        return True
+    if int(x.shape[0]) != n:
+        return True
+    for t in others:
+        if t is not None and (not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32
+                              or tuple(t.shape) != tuple(x.shape) or t.device != x.device):
+            return True
+    return (not isinstance(scale, torch.Tensor) or not scale.is_cuda or scale.dtype != torch.float32
+            or scale.numel() != n or scale.requires_grad or scale.device != x.device)
+
+
+def propagate(x, fwd, bwd, scale, a=1.0, b=0.0, h=None, acc=None, c=1.0, inplace_acc=False):
+    """One K-hop propagation step of APPNP / GCNII / SSGCConv / GPRConv on a graph's dst-CSR `fwd` (reverse CSR
+    `bwd`, a dict or a callable returning one, needed for the gradient of x) as one aggregation with a row epilogue:
+        t = scale * sum_{j -> d} scale[j] * x[j]      (the rows send_u_recv with scale_src = scale_dst = scale gives)
+        y = a * t + b * h                              (b * h only when h is given; h may be x itself)
+        acc_out = acc + c * y                          (only when acc is given)
+    Every product and sum is rounded on its own, so y and acc_out are bit for bit torch's op-by-op hop on the same
+    aggregation route.  a, b: floats (rounded to float32).  c: a float, or a one-element float32 CUDA tensor (GPRConv's
+    temp[k + 1]) read on the device, whose gradient is sum(g_acc * y).  inplace_acc: write acc_out into acc when no
+    gradient is recorded (acc must then be a buffer the caller owns).
+    Returns y, or (y, acc_out) when acc is given, or None when the call is outside the fused route: x, h, acc or the
+    norm not float32 CUDA tensors of [N, D] / N elements (N = the graph's node count), a norm that requires grad, a
+    graph without edges, or a shape the kernels refuse (PGLB_EUNSUPPORTED: 16-byte rows of D > 128 elements, which the
+    copy aggregation sends to spmm_stream).  Callers then run the op-by-op hop."""
+    n = int(fwd["indptr"].shape[0]) - 1
+    if fwd.get("cols") is None or int(fwd["cols"].shape[0]) == 0:
+        return None
+    if _propagate_declines(x, n, (h, acc), scale):
+        return None
+    if isinstance(c, torch.Tensor) and (not c.is_cuda or c.dtype != torch.float32 or c.numel() != 1
+                                        or c.device != x.device):
+        return None
+    scale = scale.reshape(-1)
+    if not scale.is_contiguous():
+        scale = scale.contiguous()
+    x2 = x if x.is_contiguous() else x.contiguous()
+    h2 = None if h is None else (x2 if h is x else h.contiguous())
+    acc2 = None if acc is None else acc.contiguous()
+    # the vector kernels read h / acc rows 16 bytes at a time: a row-offset view is copied to a fresh allocation
+    if int(x.shape[1]) % 4 == 0:
+        h2 = h2 if h2 is None or _rows16(h2) else h2.clone()
+        acc2 = acc2 if acc2 is None or _rows16(acc2) else acc2.clone()
+    D = int(x.shape[1])
+    if D % 4 == 0 and D > 128 and _rows16(x2):
+        return None   # the wide-row shapes past spmm_v5 (spmm_stream) have no epilogue
+    grad = torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in (x, h, acc, c))
+    if grad:
+        return _Propagate.apply(x2, h2, acc2, c, fwd, bwd, scale, float(a), float(b))
+    acc_out = None
+    if acc2 is not None:
+        acc_out = acc2 if (inplace_acc and acc2 is acc) else torch.empty_like(acc2)
+    y = _propagate_raw(fwd, x2, scale, float(a), float(b), h2, acc2, c, acc_out)
+    if y is None:
+        return None
+    return y if acc is None else (y, acc_out)
+
+
 def classify_bcast(x_shape, y_shape):
     """Map (x feature dims, y feature dims) to a kernel broadcast mode.
     Returns (mode, head_dim) or None when y must be materialised by expand()."""
