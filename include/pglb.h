@@ -898,6 +898,31 @@ int pglb_alias_sample(const double *alias, const int64_t *events, int64_t n, int
 int pglb_alias_sample_host(const double *alias, const int64_t *events, int64_t n, int64_t count, uint64_t seed,
                            int64_t *out);
 
+/* Skip-gram negative-sampling loss, forward (csrc/sgns.cu).  Replaces the training step of the reference's walk models
+ * (SkipGramModel.forward of examples/deepwalk/model.py and examples/metapath2vec/model.py: two embedding lookups, two
+ * matmuls and BCEWithLogitsLoss on each), which materialises the [P, 1 + K, D] context rows.
+ *   emb [n_emb, ld_emb] and ctx [n_ctx, ld_ctx] float32 tables (first D columns used; ctx == emb for a shared table),
+ *   src[P] and dsts[P, 1 + K] int64 row ids (column 0 the positive, 1..K the negatives), every id inside its table
+ *   (not checked here).  With s[p, j] = <emb[src[p]], ctx[dsts[p, j]]>:
+ *     *loss   = ( mean_p softplus(-s[p, 0]) + mean_{p, k >= 1} softplus(s[p, k]) ) / 2
+ *     c[p, 0] = -sigmoid(-s[p, 0]) / (2P),  c[p, k] = sigmoid(s[p, k]) / (2PK)     (float32 [P, 1 + K], = d loss / d s)
+ *     w[p]    = sum_j c[p, j] ctx[dsts[p, j]]                                  (float32 [P, ldw], first D columns)
+ *   softplus(x) = max(x, 0) + log1p(exp(-|x|)); saturated logits give finite values.  c and w are both given (training)
+ *   or both NULL (loss only).  The loss is the sum of fixed-order per-block partials, then a one-block fixed-order sum:
+ *   bit-identical run to run.  Two launches.  Any D >= 1; rows are read 16 bytes at a time when D, ld_emb, ld_ctx (and
+ *   ldw) are multiples of 4 and the tables (and w) are 16-byte aligned, and held in registers up to D = 512 (256 when
+ *   read 4 bytes at a time); wider rows stream through a warp per pair.
+ *   Refused before any CUDA call: a NULL table, id array, loss or workspace (PGLB_EINVAL); P, K, D, n_emb or n_ctx < 1
+ *   (PGLB_EINVAL); ld_emb, ld_ctx or (training) ldw < D (PGLB_ESHAPE); only one of c and w (PGLB_EINVAL); an output
+ *   overlapping an input or another output (PGLB_EINVAL); ws below pglb_sgns_fwd_ws(P) bytes or not 8-byte aligned
+ *   (PGLB_EWORKSPACE).
+ * The gradients are segment sums of these by node id, and run on the aggregation entries: d emb[n] = g sum over pairs
+ * with src[p] = n of w[p]; d ctx[m] = g sum over (p, j) with dsts[p, j] = m of c[p, j] emb[src[p]]. */
+int pglb_sgns_fwd_ws(int64_t P, size_t *ws_bytes);
+int pglb_sgns_fwd_f32(const float *emb, int64_t n_emb, int64_t ld_emb, const float *ctx, int64_t n_ctx, int64_t ld_ctx,
+                      const int64_t *src, const int64_t *dsts, int64_t P, int64_t K, int64_t D, float *loss, float *c,
+                      float *w, int64_t ldw, void *ws, size_t ws_bytes, void *stream);
+
 /* ------------------------------------------------------------------------------------
  * Graph-level readouts (csrc/readout.cu).  Every entry is keyed by a segment CSR indptr[B + 1] (device int64,
  * non-decreasing, indptr[0] = 0, indptr[B] = N): segment g is the contiguous rows indptr[g] .. indptr[g + 1] - 1 (a

@@ -100,6 +100,9 @@ _SIGS = {
     "pglb_alias_build_host": (c_int, [_p, _i64, _p, _p]),
     "pglb_alias_sample": (c_int, [_p, _p, _i64, _i64, _u64, _p, _p]),
     "pglb_alias_sample_host": (c_int, [_p, _p, _i64, _i64, _u64, _p]),
+    "pglb_sgns_fwd_ws": (c_int, [_i64, POINTER(c_size_t)]),
+    "pglb_sgns_fwd_f32": (c_int, [_p, _i64, _i64, _p, _i64, _i64, _p, _p, _i64, _i64, _i64, _p, _p, _p, _i64, _p,
+                                  c_size_t, _p]),
     "pglb_attn_readout_ws": (c_int, [_i64, _i64, _i64, _i64, POINTER(c_size_t)]),
     "pglb_attn_readout_f32": (c_int, [_p, _i64, _i64, _p, _i64, _i64, _p, _p, _p, _p, _p, c_size_t, _p]),
     "pglb_attn_readout_bwd_f32": (c_int, [_p, _i64, _i64, _p, _i64, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p,

@@ -258,6 +258,176 @@ def alias_sample(alias, events, count, seed):
     return out
 
 
+# skip-gram negative-sampling loss (csrc/sgns.cu forward; the backward on csr_build and the aggregation)
+# ------------------------------------------------------------------------------------------
+
+
+def _sgns_check_ids(src, dsts):
+    """The id checks that need no device: dtype, rank, K >= 1 and matching P."""
+    for name, t in (("src", src), ("dsts", dsts)):
+        if not isinstance(t, torch.Tensor) or t.dtype not in (torch.int32, torch.int64):
+            raise ValueError("skip_gram_loss: %s must be an int32 or int64 tensor, got %s"
+                             % (name, getattr(t, "dtype", type(t).__name__)))
+    if not (src.dim() == 1 or (src.dim() == 2 and src.shape[1] == 1)):
+        raise ValueError("skip_gram_loss: src must be [P] or [P, 1], got %s" % (tuple(src.shape),))
+    if dsts.dim() != 2 or dsts.shape[1] < 2:
+        raise ValueError("skip_gram_loss: dsts must be [P, 1 + K] with K >= 1, got %s" % (tuple(dsts.shape),))
+    P = int(src.shape[0])
+    if P < 1 or int(dsts.shape[0]) != P:
+        raise ValueError("skip_gram_loss: src has %d pairs and dsts %d; both need at least one" % (P, dsts.shape[0]))
+
+
+def _sgns_ids(src, dsts, n_emb, n_ctx):
+    """src / dsts as contiguous int64 [P] / [P, 1 + K], after one read-back of the ids' extremes: IndexError outside
+    the tables, before any kernel dereferences a row."""
+    lo_s, hi_s = torch.aminmax(src)
+    lo_d, hi_d = torch.aminmax(dsts)
+    lo_s, hi_s, lo_d, hi_d = torch.stack([lo_s.long(), hi_s.long(), lo_d.long(), hi_d.long()]).tolist()
+    if lo_s < 0 or hi_s >= n_emb:
+        raise IndexError("skip_gram_loss: src ids span [%d, %d], outside the centre table of %d rows"
+                         % (lo_s, hi_s, n_emb))
+    if lo_d < 0 or hi_d >= n_ctx:
+        raise IndexError("skip_gram_loss: dsts ids span [%d, %d], outside the context table of %d rows"
+                         % (lo_d, hi_d, n_ctx))
+    return _i64(src).reshape(-1).contiguous(), _i64(dsts).contiguous()
+
+
+def _sgns_table(t):
+    """t as rows of unit column stride that do not overlap (ld >= D), copied only when it is not already so: an
+    expanded or otherwise overlapping view is read from a contiguous copy."""
+    return t if t.stride(1) == 1 and t.stride(0) >= t.shape[1] else t.contiguous()
+
+
+def _sgns_fwd_raw(emb, ctx, src, dsts, train):
+    """pglb_sgns_fwd_f32: (loss, c, w); c [P, 1 + K] and w [P, D] only when train."""
+    P, J = dsts.shape
+    D = int(emb.shape[1])
+    dev = emb.device
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    c = torch.empty((P, J), dtype=torch.float32, device=dev) if train else None
+    w = torch.empty((P, D), dtype=torch.float32, device=dev) if train else None
+    need = ctypes.c_size_t(0)
+    check(lib.pglb_sgns_fwd_ws(P, ctypes.byref(need)))
+    ws = workspace(dev, need.value)
+    with torch.cuda.device(dev):
+        check(lib.pglb_sgns_fwd_f32(_ptr(emb), int(emb.shape[0]), emb.stride(0), _ptr(ctx), int(ctx.shape[0]),
+                                    ctx.stride(0), _ptr(src), _ptr(dsts), P, J - 1, D, _ptr(loss), _ptr(c), _ptr(w),
+                                    D, _ptr(ws), ws.numel(), _stream()))
+    return loss, c, w
+
+
+def _touched(indptr, num_edges):
+    """Rows of a key-sorted CSR that hold a slot, and the CSR compacted to them: (rows [R], indptr [R + 1])."""
+    rows, _ = segment_ids_from_indptr(indptr, num_edges)
+    return rows, torch.cat([indptr[rows], indptr[-1:]])
+
+
+def _sgns_grads(g, emb, src, dsts, c, w, n_emb, n_ctx, shared, sparse, need_emb, need_ctx):
+    """d loss / d emb and d ctx (one tensor for a shared table) as segment sums by node id:
+    d emb[n] = g sum_{p: src[p] = n} w[p] over the CSR of the P keys src (slots -> pairs);
+    d ctx[m] = g sum_{(p, j): dsts[p, j] = m} c[p, j] emb[src[p]] over the CSR of the P (1 + K) keys dsts, with the
+    edge operand g c.  csr_build is stable and the aggregation sums every row in slot order: no atomics, so the
+    gradients are bit-identical run to run.  sparse: coalesced COO gradients over the touched rows only."""
+    P, J = dsts.shape
+    D = int(emb.shape[1])
+    dev = emb.device
+    E = P * J
+    ge = gc = None
+    if need_emb or shared:
+        _, _, _, pair, ip_e = csr_build(src, src, n_emb)
+        # the upstream scalar as a per-slot operand of stride 0: stays on the device
+        g_slot = g.reshape(1, 1).expand(P, 1)
+    if need_ctx or shared:
+        _, col_c, _, slot_c, ip_c = csr_build(dsts.reshape(-1), src.repeat_interleave(J), n_ctx)
+        gcoef = (c.reshape(-1) * g).reshape(E, 1)
+
+    def emb_part(indptr, rows, out, acc):
+        return _spmm_raw(indptr, pair, w, rows, "sum", y2=g_slot, y_bcast=BCAST_SCALAR, msg_op="mul", num_edges=P,
+                         out=out, accumulate=acc)
+
+    def ctx_part(indptr, rows, out, acc):
+        return _spmm_raw(indptr, col_c, emb, rows, "sum", eid=slot_c, y2=gcoef, y_bcast=BCAST_SCALAR, msg_op="mul",
+                         num_edges=E, out=out, accumulate=acc)
+
+    if shared:
+        if not sparse:
+            out = emb_part(ip_e, n_emb, None, False)
+            return ctx_part(ip_c, n_emb, out, True), None
+        rows, _ = segment_ids_from_indptr(ip_e + ip_c, P + E)     # rows touched in either role
+        cip_e = torch.cat([ip_e[rows], ip_e[-1:]])
+        cip_c = torch.cat([ip_c[rows], ip_c[-1:]])
+        vals = emb_part(cip_e, int(rows.numel()), None, False)
+        vals = ctx_part(cip_c, int(rows.numel()), vals, True)
+        return torch.sparse_coo_tensor(rows[None], vals, (n_emb, D), is_coalesced=True, check_invariants=False), None
+    if need_emb:
+        if sparse:
+            rows, cip = _touched(ip_e, P)
+            ge = torch.sparse_coo_tensor(rows[None], emb_part(cip, int(rows.numel()), None, False), (n_emb, D),
+                                         is_coalesced=True, check_invariants=False)
+        else:
+            ge = emb_part(ip_e, n_emb, None, False)
+    if need_ctx:
+        if sparse:
+            rows, cip = _touched(ip_c, E)
+            gc = torch.sparse_coo_tensor(rows[None], ctx_part(cip, int(rows.numel()), None, False), (n_ctx, D),
+                                         is_coalesced=True, check_invariants=False)
+        else:
+            gc = ctx_part(ip_c, n_ctx, None, False)
+    return ge, gc
+
+
+class _SkipGramLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, emb, ctx_table, src, dsts, sparse, train):
+        shared = ctx_table is None
+        table = emb if shared else ctx_table
+        loss, c, w = _sgns_fwd_raw(emb, table, src, dsts, train)
+        if train:
+            ctx.save_for_backward(emb, src, dsts, c, w)
+            ctx.meta = (int(emb.shape[0]), int(table.shape[0]), shared, bool(sparse))
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        emb, src, dsts, c, w = ctx.saved_tensors
+        n_emb, n_ctx, shared, sparse = ctx.meta
+        ge, gc = _sgns_grads(g, emb, src, dsts, c, w, n_emb, n_ctx, shared, sparse,
+                             ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        return ge, gc, None, None, None, None
+
+
+@f64_through
+def _skip_gram_loss_f32(emb, ctx, src, dsts, sparse):
+    # training writes c and w for the backward; inside torch.no_grad(), or when no table needs a gradient, the kernel
+    # writes the loss only (needs_input_grad inside forward follows requires_grad, not grad mode)
+    train = torch.is_grad_enabled() and (emb.requires_grad or (ctx is not None and ctx.requires_grad))
+    return _SkipGramLoss.apply(_sgns_table(emb), None if ctx is None else _sgns_table(ctx), src, dsts, sparse, train)
+
+
+def skip_gram_loss(emb, ctx, src, dsts, sparse=False):
+    """The skip-gram negative-sampling loss of the reference's SkipGramModel on the fused kernel (pglb_sgns_fwd_f32):
+    (BCEWithLogits(<emb[src], ctx[dsts[:, 0]]>, 1) + BCEWithLogits(<emb[src], ctx[dsts[:, 1:]]>, 0)) / 2, mean
+    reduction.  ``ctx is emb`` is a shared table, which receives both roles' gradients.  float32 tables (float64
+    through f64_through); int32 / int64 CUDA ids.  sparse: the gradients are coalesced sparse COO tensors over the
+    touched rows (for torch.optim.SparseAdam, SGD, Adagrad), else dense [N, D].  Every check precedes any launch:
+    16-bit or other non-float32/64 tables raise TypeError; float or bool ids, wrong ranks and K = 0 raise ValueError;
+    ids outside their table raise IndexError (one read-back of the ids' extremes)."""
+    shared = ctx is emb
+    for name, t in (("emb", emb), ("ctx", ctx)):
+        if t.dtype not in (torch.float32, torch.float64):
+            raise TypeError("skip_gram_loss: float32 or float64 tables, got %s for %s" % (t.dtype, name))
+        if t.dim() != 2:
+            raise ValueError("skip_gram_loss: %s must be a 2-D table, got %s" % (name, tuple(t.shape)))
+    if emb.shape[1] != ctx.shape[1] or emb.shape[1] < 1:
+        raise ValueError("skip_gram_loss: the tables' widths differ or are 0 (%d, %d)" % (emb.shape[1], ctx.shape[1]))
+    _sgns_check_ids(src, dsts)
+    require_cuda(emb, ctx, src, dsts)
+    if len({emb.device, ctx.device, src.device, dsts.device}) != 1:
+        raise ValueError("skip_gram_loss: the tables and ids must be on one device")
+    src, dsts = _sgns_ids(src, dsts, int(emb.shape[0]), int(ctx.shape[0]))
+    return _skip_gram_loss_f32(emb, None if shared else ctx, src, dsts, sparse)
+
+
 # graph-level readouts (csrc/readout.cu)
 # ------------------------------------------------------------------------------------------
 
